@@ -45,6 +45,13 @@ CASES = [
     {"name": "depth_only_invalid_pose", "wh": [128, 96], "frames": 6, "seed": 22, "loop": 90, "noise": 0.0, "drop": 0.1, "inv": 4, "color": False, "over": {}},
     {"name": "weighted", "wh": [80, 60], "frames": 9, "seed": 23, "loop": 3000, "noise": 0.5, "drop": 0.0, "inv": 0, "color": True,
      "over": {"weight_sample": 10, "weight_max": 30}},
+    # per-sample weight past the 512-entry reciprocal table of the integrate kernel (w1 up to 1500)
+    {"name": "heavy_weight_sample", "wh": [64, 48], "frames": 4, "seed": 24, "loop": 300, "noise": 0.5, "drop": 0.01, "inv": 0, "color": True,
+     "over": {"weight_sample": 1000}},
+    {"name": "voxel_1mm", "wh": [24, 18], "frames": 3, "seed": 25, "loop": 300, "noise": 0.0, "drop": 0.0, "inv": 0, "color": True,
+     "over": {"voxel_size": 0.001}},
+    {"name": "voxel_2cm_no_trunc_scale", "wh": [72, 54], "frames": 5, "seed": 26, "loop": 100, "noise": 1.0, "drop": 0.02, "inv": 3, "color": False,
+     "over": {"voxel_size": 0.02, "trunc_scale": 0.0}},
 ]
 
 if __name__ == "__main__":
