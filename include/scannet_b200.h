@@ -346,6 +346,56 @@ int  scn_fuse_many(const char* const* sens_paths, const char* const* out_plys /*
 /* `fuse <params.txt> <file.sens> [out.ply]` — the recons/improve stage contract; `fuse --gpus N <params.txt> a.sens b.sens ...` */
 int  scn_fuse_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Mesh cleaning (DESIGN.md §6f): the first step of the `decimate` stage, `meshlabserver -i <id>_vh.ply -o <id>_vh_clean.ply
+ * -m vc -s clean.mlx` (Server/scan_processor.py:142-146, Server/tools/meshclean/clean.mlx), stated as mLib's MeshData
+ * operators (external/mLib/include/core-mesh/meshData.cpp) and run in clean.mlx's order, every step on the GPU:
+ *   1. merge close vertices   mergeCloseVertices(t, approx=false) :217-289, then removeDegeneratedFaces :293-318
+ *   2. duplicate faces        removeDuplicateFaces :40-104 (first face of every sorted index triple survives)
+ *   3. isolated pieces        removeIsolatedPieces :407-454 + removeIsolatedVertices :324-360 (vertex renumbering by first
+ *                             appearance in face/corner order; unreferenced vertices dropped)
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define SCN_CLEAN_SKIP_MERGE  1u
+#define SCN_CLEAN_SKIP_DEDUP  2u
+#define SCN_CLEAN_SKIP_PIECES 4u
+typedef struct {
+  float    merge_threshold;     /* t: vertices closer than t (d^2 < t*t) merge; clean.mlx 0.0010689 */
+  uint32_t min_piece_vertices;  /* a face survives only if its piece has >= this many vertices (mLib's unit; 0 = off) */
+  uint32_t min_piece_faces;     /* ... and >= this many faces after steps 1-2 (clean.mlx MinComponentSize 7500; 0 = off) */
+  uint32_t flags;               /* SCN_CLEAN_SKIP_* */
+} scn_mesh_clean_params;
+typedef struct scn_mesh_clean_report {
+  uint64_t vertices_in, faces_in, vertices_out, faces_out;
+  uint64_t vertices_merged;            /* step 1: vertices that mapped onto an earlier representative */
+  uint64_t merge_components;           /* step 1: components of >= 2 vertices of the proximity graph (pairs in neighbouring cells, d^2 < t^2) */
+  uint64_t largest_merge_component;    /* step 1: vertices in the largest such component (1 when nothing is within t) */
+  uint64_t degenerate_faces;           /* step 1: faces with a repeated index after the remap */
+  uint64_t duplicate_faces;            /* step 2 */
+  uint64_t pieces_total;               /* step 3: pieces with at least one face */
+  uint64_t pieces_removed;
+  uint64_t faces_in_removed_pieces;
+  double   upload_ms, merge_ms, dedup_ms, pieces_ms, download_ms, total_ms;   /* CUDA events on the call's stream */
+} scn_mesh_clean_report_t;
+void   scn_mesh_clean_default_params(scn_mesh_clean_params* p);
+size_t scn_mesh_clean_report_sizeof(void);
+/* Reads a MeshLab FilterScript made of clean.mlx's filters (Merge Close Vertices / Remove Duplicate Faces / Remove Isolated
+ * pieces (wrt Face Num.) / Remove Unreferenced Vertex, in that order, any of them may be absent): sets merge_threshold,
+ * min_piece_faces and the SKIP flags of *p.  Any other filter (e.g. simplify.mlx's Quadric Edge Collapse Decimation) gives
+ * SCN_ERR_UNSUPPORTED naming it. */
+int  scn_mesh_clean_params_from_mlx(const char* path, scn_mesh_clean_params* p);
+/* rgb (n_verts*3) may be NULL; then *rgb_out is NULL.  Outputs are malloc'ed (scn_free); report may be NULL.
+ * SCN_ERR_ARG: a face index >= n_verts; unless the merge is skipped also t <= 0 or NaN, a non-finite coordinate, or
+ * |v_i / t| >= 2^31 (the cell's int conversion would be undefined). */
+int  scn_mesh_clean(const float* xyz, const uint8_t* rgb, uint64_t n_verts, const uint32_t* tri, uint64_t n_faces,
+                    const scn_mesh_clean_params* params, float** xyz_out, uint8_t** rgb_out, uint32_t** tri_out,
+                    uint64_t* n_verts_out, uint64_t* n_faces_out, scn_mesh_clean_report_t* report);
+/* scn_mesh_load plus per-vertex colour: *rgb (n_verts*3, malloc'ed) when the vertex element has uchar red, green and blue,
+ * else NULL.  Same acceptance rules as scn_mesh_load. */
+int  scn_mesh_load_rgb(const char* path, float** xyz, uint8_t** rgb, uint64_t* n_verts, uint32_t** tri, uint64_t* n_faces);
+/* `meshclean -i in.ply -o out.ply [-m vc] [-s script.mlx]`: the meshlabserver arguments of scan_processor.py:143.  Without -s
+ * the clean.mlx defaults apply; without `-m vc` the output carries no colour (white). */
+int  scn_meshclean_main(int argc, const char** argv);
+
 #ifdef __cplusplus
 }
 #endif

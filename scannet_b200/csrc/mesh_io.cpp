@@ -59,7 +59,8 @@ inline int64_t as_int(const uint8_t* p, PType t, bool big) {
     case T_I32: return (int32_t)u; case T_U32: return (uint32_t)u; default: return 0; }
 }
 
-int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint32_t>& tri) {
+// rgb != nullptr: also the vertex colour when the vertex element has uchar red, green and blue (else rgb stays empty)
+int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint32_t>& tri, std::vector<uint8_t>* rgb = nullptr) {
   // the file is mapped, not read: a 2 M-vertex mesh is 84 MB and the arrays below are the only copy that is needed
   struct FileView {
     const uint8_t* p = nullptr; size_t n = 0; bool mapped = false; std::vector<uint8_t> own;
@@ -123,6 +124,16 @@ int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint3
     have_xyz = got == 3;
   }
   xyz.clear(); tri.clear();
+  bool want_rgb = false;
+  auto rgb_slot = [](const std::string& n) { return n == "red" ? 0 : n == "green" ? 1 : n == "blue" ? 2 : -1; };
+  if (rgb) {
+    rgb->clear();
+    for (const PElem& el : elems) if (el.name == "vertex") {
+      int got = 0;
+      for (const PProp& p : el.props) if (!p.is_list && p.type == T_U8 && rgb_slot(p.name) >= 0) ++got;
+      want_rgb = got == 3 && have_xyz;
+    }
+  }
   const uint8_t* d = buf.data(); const size_t n = buf.size();
   if (binary) {
     for (const PElem& el : elems) {
@@ -135,6 +146,7 @@ int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint3
       for (const PProp& p : el.props) min_rec += p.is_list ? psize(p.list_type) : psize(p.type);
       if (el.count > (n - std::min(pos, n)) / std::max<size_t>(min_rec, 1)) return scn::fail(SCN_ERR_FORMAT, "PLY body truncated");
       if (is_v) xyz.resize(el.count * 3);
+      if (is_v && want_rgb) rgb->resize(el.count * 3);
       if (is_f) tri.reserve(el.count * 3);
       if (fixed) {
         if (rec * el.count > n - pos) return scn::fail(SCN_ERR_FORMAT, "PLY body truncated");
@@ -148,6 +160,11 @@ int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint3
             const uint8_t* r = d + pos + i * rec;
             uint32_t a = (uint32_t)load_le(r + ox, 4, big), b = (uint32_t)load_le(r + oy, 4, big), c = (uint32_t)load_le(r + oz, 4, big);
             memcpy(&xyz[3 * i], &a, 4); memcpy(&xyz[3 * i + 1], &b, 4); memcpy(&xyz[3 * i + 2], &c, 4);
+          }
+          if (want_rgb) {
+            size_t oc[3] = {0, 0, 0}; o = 0;
+            for (const PProp& p : el.props) { const int k = rgb_slot(p.name); if (k >= 0 && p.type == T_U8) oc[k] = o; o += psize(p.type); }
+            for (size_t i = 0; i < el.count; ++i) for (int k = 0; k < 3; ++k) (*rgb)[3 * i + k] = d[pos + i * rec + oc[k]];
           }
         }
         pos += rec * el.count;
@@ -167,6 +184,7 @@ int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint3
             if (!p.is_list) {
               if (pos + psize(p.type) > n) return scn::fail(SCN_ERR_FORMAT, "PLY body truncated");
               if (is_v && (p.name == "x" || p.name == "y" || p.name == "z")) { uint32_t a = (uint32_t)load_le(d + pos, 4, big); memcpy(&xyz[3 * i + (p.name[0] - 'x')], &a, 4); }
+              if (is_v && want_rgb && p.type == T_U8 && rgb_slot(p.name) >= 0) (*rgb)[3 * i + rgb_slot(p.name)] = d[pos];
               pos += psize(p.type);
             } else {
               if (p.list_type == T_BAD || p.list_type == T_F32 || p.list_type == T_F64) return scn::fail(SCN_ERR_FORMAT, "invalid ply list count type");
@@ -191,9 +209,11 @@ int load_ply(const std::string& path, std::vector<float>& xyz, std::vector<uint3
       const bool is_v = el.name == "vertex" && have_xyz, is_f = el.name == "face" && !face_prop.empty();
       if (el.count > n - std::min(pos, n)) return scn::fail(SCN_ERR_FORMAT, "PLY body truncated");   // >= 1 byte per record
       if (is_v) xyz.resize(el.count * 3);
+      if (is_v && want_rgb) rgb->resize(el.count * 3);
       for (size_t i = 0; i < el.count; ++i) for (const PProp& p : el.props) {
         if (!p.is_list) {
           if (is_v && (p.name == "x" || p.name == "y" || p.name == "z")) { float v = 0; is >> v; xyz[3 * i + (p.name[0] - 'x')] = v; }   // ply_cast_ascii<float>
+          else if (is_v && want_rgb && p.type == T_U8 && rgb_slot(p.name) >= 0) { int v = 0; is >> v; (*rgb)[3 * i + rgb_slot(p.name)] = (uint8_t)v; }
           else { std::string s; is >> s; }
         } else {
           long long cnt = 0; is >> cnt;
@@ -353,6 +373,28 @@ int scn_mesh_load(const char* path, float** xyz, uint64_t* n_verts, uint32_t** t
   *xyz = (float*)malloc(std::max<size_t>(1, v.size() * 4)); *tri = (uint32_t*)malloc(std::max<size_t>(1, t.size() * 4));
   if (!*xyz || !*tri) return scn::fail(SCN_ERR_ARG, "out of memory");
   memcpy(*xyz, v.data(), v.size() * 4); memcpy(*tri, t.data(), t.size() * 4);
+  return SCN_OK;
+}
+
+int scn_mesh_load_rgb(const char* path, float** xyz, uint8_t** rgb, uint64_t* n_verts, uint32_t** tri, uint64_t* n_faces) {
+  if (!path || !xyz || !rgb || !n_verts || !tri || !n_faces) return scn::fail(SCN_ERR_ARG, "null argument");
+  *xyz = nullptr; *rgb = nullptr; *tri = nullptr; *n_verts = 0; *n_faces = 0;
+  const std::string p = path;
+  std::vector<float> v; std::vector<uint32_t> t; std::vector<uint8_t> c;
+  int rc;
+  try {
+    if (ends_with(p, ".ply") || ends_with(p, ".PLY")) rc = load_ply(p, v, t, &c);
+    else if (ends_with(p, ".obj") || ends_with(p, ".OBJ")) rc = load_obj(p, v, t);
+    else rc = SCN_OK;
+  } catch (const std::bad_alloc&) { return scn::fail(SCN_ERR_FORMAT, "mesh file %s: out of memory while parsing", path);
+  } catch (const std::exception& e) { return scn::fail(SCN_ERR_FORMAT, "mesh file %s: %s", path, e.what()); }
+  if (rc) return rc;
+  *n_verts = v.size() / 3; *n_faces = t.size() / 3;
+  *xyz = (float*)malloc(std::max<size_t>(1, v.size() * 4)); *tri = (uint32_t*)malloc(std::max<size_t>(1, t.size() * 4));
+  if (!c.empty()) *rgb = (uint8_t*)malloc(c.size());
+  if (!*xyz || !*tri || (!c.empty() && !*rgb)) return scn::fail(SCN_ERR_ARG, "out of memory");
+  memcpy(*xyz, v.data(), v.size() * 4); memcpy(*tri, t.data(), t.size() * 4);
+  if (!c.empty()) memcpy(*rgb, c.data(), c.size());
   return SCN_OK;
 }
 
