@@ -33,6 +33,7 @@ $(BINDIR)/%: scannet_b200/tools/%_main.cpp $(LIB) | $(BINDIR)
 oracle:
 	$(MAKE) -C oracle all
 	$(MAKE) -C oracle -f meshclean.mk all
+	$(MAKE) -C oracle -f meshsimplify.mk all
 
 $(OBJDIR) $(LIBDIR) $(BINDIR):
 	mkdir -p $@

@@ -396,6 +396,47 @@ int  scn_mesh_load_rgb(const char* path, float** xyz, uint8_t** rgb, uint64_t* n
  * the clean.mlx defaults apply; without `-m vc` the output carries no colour (white). */
 int  scn_meshclean_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Mesh decimation (DESIGN.md §6g): the second and third steps of the `decimate` stage, `meshlabserver -i <id>_vh_clean.ply
+ * -o <id>_vh_clean_1.ply -m vc -s simplify.mlx` and again into <id>_vh_clean_2.ply (Server/scan_processor.py:144-145).
+ * Quadric edge-collapse decimation (Garland-Heckbert quadrics, binary64) in deterministic rounds of independent collapses,
+ * this repository's own spec: MeshLab/VCG is not in the reference tree and the result is NOT MeshLab's mesh.  Then AutoClean
+ * (duplicate faces, unreferenced vertices) and the script's clean filters (scn_mesh_clean's steps), every step on the GPU.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct {
+  uint64_t target_faces;        /* TargetFaceNum: the face target when target_perc == 0 */
+  double   target_perc;         /* TargetPerc in [0, 1]: target = floor(faces_in * target_perc) when != 0 (simplify.mlx 0.2) */
+  double   quality_thr;         /* QualityThr >= 0: collapses leaving a triangle of quality q < thr cost thr / max(q, 1e-6) times more (0.3) */
+} scn_mesh_simplify_params;
+typedef struct scn_mesh_simplify_report {
+  uint64_t vertices_in, faces_in, vertices_out, faces_out;
+  uint64_t target_faces;               /* the face target of the rounds */
+  uint64_t rounds;                     /* rounds that applied at least one collapse */
+  uint64_t collapses;
+  uint64_t faces_collapsed;            /* faces removed by the collapses */
+  uint64_t autoclean_duplicate_faces;  /* AutoClean: duplicate faces removed after the rounds */
+  uint64_t max_vertex_faces;           /* the largest number of face corners at one vertex, over all rounds */
+  double   upload_ms, quadrics_ms, rounds_ms, autoclean_ms, clean_ms, download_ms, total_ms;   /* CUDA events on the call's stream */
+  scn_mesh_clean_report_t clean;       /* the clean filters after AutoClean (sizes and counters; all zero when `after` is NULL) */
+} scn_mesh_simplify_report_t;
+/* simplify.mlx: TargetPerc 0.2, QualityThr 0.3; *after (may be NULL): Merge Close Vertices 0.0010689, Remove Duplicate Faces,
+ * Remove Isolated pieces < 1000 faces, Remove Unreferenced Vertex */
+void   scn_mesh_simplify_default_params(scn_mesh_simplify_params* p, scn_mesh_clean_params* after);
+size_t scn_mesh_simplify_report_sizeof(void);
+/* Reads a FilterScript whose first filter is Quadric Edge Collapse Decimation (once) followed by clean.mlx's filters (read as
+ * scn_mesh_clean_params_from_mlx does, into *after).  The decimation's booleans must have simplify.mlx's values
+ * (OptimalPlacement and AutoClean true, the others false) and BoundaryWeight 1: anything else, an unknown parameter or a script
+ * without the decimation gives SCN_ERR_UNSUPPORTED naming it. */
+int  scn_mesh_simplify_params_from_mlx(const char* path, scn_mesh_simplify_params* p, scn_mesh_clean_params* after);
+/* Shaped like scn_mesh_clean; after == NULL runs no clean filter.  SCN_ERR_ARG: a face index >= n_verts, a non-finite
+ * coordinate, target_perc NaN or outside [0, 1], quality_thr NaN or negative, and the refusals of scn_mesh_clean's filters. */
+int  scn_mesh_simplify(const float* xyz, const uint8_t* rgb, uint64_t n_verts, const uint32_t* tri, uint64_t n_faces,
+                       const scn_mesh_simplify_params* params, const scn_mesh_clean_params* after, float** xyz_out, uint8_t** rgb_out,
+                       uint32_t** tri_out, uint64_t* n_verts_out, uint64_t* n_faces_out, scn_mesh_simplify_report_t* report);
+/* `meshsimplify -i in.ply -o out.ply [-m vc] [-s simplify.mlx]`: the meshlabserver arguments of scan_processor.py:144-145.
+ * Without -s the simplify.mlx defaults apply; without `-m vc` the output carries no colour (white). */
+int  scn_meshsimplify_main(int argc, const char** argv);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,31 +22,19 @@
 #include <cstring>
 #include <vector>
 
+#include "meshclean_steps.h"
 #include "radix_sort.cuh"
 #include "scan.cuh"
 #include "scn_common.h"
 
-namespace {
+namespace scn::mc {
 
 using scn::bits_for;
 using scn::k_iota;
 using scn::radix_sort_pairs;
 using scn::rs_hist_elems;
 
-struct DBuf {                      // cudaMalloc with scope lifetime
-  void* p = nullptr;
-  DBuf() = default;
-  DBuf(const DBuf&) = delete;
-  DBuf& operator=(const DBuf&) = delete;
-  ~DBuf() { if (p) cudaFree(p); }
-  template <typename T> T* as() const { return (T*)p; }
-  bool alloc(size_t bytes) { if (p) { cudaFree(p); p = nullptr; } return cudaMalloc(&p, bytes ? bytes : 4) == cudaSuccess; }
-  void swap(DBuf& o) { std::swap(p, o.p); }
-};
-#define MC_ALLOC(buf, bytes) do { if (!(buf).alloc(bytes)) { cudaGetLastError(); return scn::fail(SCN_ERR_CUDA, "cudaMalloc(%zu) failed (%s:%d)", (size_t)(bytes), __FILE__, __LINE__); } } while (0)
-
 enum : unsigned { ERR_INDEX = 1u, ERR_CELL = 2u };
-inline unsigned grid_for(size_t n) { return (unsigned)((n + 255) / 256); }
 __device__ __forceinline__ size_t tid() { return blockIdx.x * (size_t)blockDim.x + threadIdx.x; }
 
 __global__ void k_check_faces(const unsigned* __restrict__ tri, size_t nC, unsigned nV, unsigned* err) {
@@ -279,6 +267,10 @@ __global__ void k_piece_keep(const unsigned* __restrict__ tri, unsigned nF, cons
   const unsigned r = root[tri[3 * f]];
   keep[f] = piece_kept(vcount[r], fcount[r], min_v, min_f) ? 1u : 0u;
 }
+__global__ void k_mark_used(const unsigned* __restrict__ tri, unsigned nC, unsigned* __restrict__ used) {
+  const size_t c = tid();
+  if (c < nC) used[tri[c]] = 1u;
+}
 __global__ void k_first_corner(const unsigned* __restrict__ tri, unsigned nC, unsigned* __restrict__ first) {
   const size_t c = tid();
   if (c < nC) atomicMin(&first[tri[c]], (unsigned)c);
@@ -302,26 +294,6 @@ __global__ void k_renumber(const unsigned* __restrict__ tri, unsigned nC, const 
 }
 
 // ------------------------------------------------------------------------------------------ host driver
-struct Mesh {                         // the current mesh, in device memory
-  DBuf xyz, rgb, tri;
-  unsigned nV = 0, nF = 0;
-  bool has_rgb = false;
-};
-
-struct Scratch {                      // radix-sort pairs and scan scratch, grown on demand
-  DBuf k0, v0, k1, v1, hist, scr;
-  size_t cap_pairs = 0, cap_scan = 0;
-  int ensure(size_t n, size_t scan_n) {          // sorts of n pairs, scans of up to scan_n elements
-    if (n > cap_pairs) {
-      MC_ALLOC(k0, n * 4); MC_ALLOC(v0, n * 4); MC_ALLOC(k1, n * 4); MC_ALLOC(v1, n * 4); MC_ALLOC(hist, rs_hist_elems(n) * 4);
-      cap_pairs = n;
-    }
-    const size_t need = scn::scan_scratch_elems(std::max(rs_hist_elems(cap_pairs), scan_n));
-    if (need > cap_scan) { MC_ALLOC(scr, need * 4); cap_scan = need; }
-    return SCN_OK;
-  }
-};
-
 int read_u32(const unsigned* d, unsigned* h, size_t n, cudaStream_t st) {
   SCN_CUDA_TRY(cudaMemcpyAsync(h, d, n * 4, cudaMemcpyDeviceToHost, st));
   SCN_CUDA_TRY(cudaStreamSynchronize(st));
@@ -482,15 +454,53 @@ int step_pieces(Mesh& m, unsigned min_v, unsigned min_f, Scratch& s, scn_mesh_cl
   return SCN_OK;
 }
 
-struct Stream {
-  cudaStream_t s = nullptr;
-  cudaEvent_t ev[6] = {};
-  ~Stream() { for (auto e : ev) if (e) cudaEventDestroy(e); if (s) cudaStreamDestroy(s); }
-};
+int drop_unreferenced(Mesh& m, Scratch& s, cudaStream_t st, unsigned* h_small) {
+  const unsigned n = m.nV, nC = 3 * m.nF;
+  if (int rc = s.ensure(1, (size_t)n + 1)) return rc;
+  DBuf used, newid, ident, keep, otri, oxyz, orgb;
+  MC_ALLOC(used, (size_t)n * 4); MC_ALLOC(newid, ((size_t)n + 1) * 4); MC_ALLOC(ident, (size_t)n * 4); MC_ALLOC(keep, (size_t)m.nF * 4);
+  MC_ALLOC(otri, (size_t)nC * 4);
+  unsigned nV2 = 0;
+  if (n) {
+    SCN_CUDA_TRY(cudaMemsetAsync(used.p, 0, (size_t)n * 4, st));
+    if (nC) k_mark_used<<<grid_for(nC), 256, 0, st>>>(m.tri.as<unsigned>(), nC, used.as<unsigned>());
+    k_iota<<<grid_for(n), 256, 0, st>>>(ident.as<unsigned>(), n);
+    scn::exclusive_scan_u32(used.as<unsigned>(), newid.as<unsigned>(), n, s.scr.as<unsigned>(), st);
+    if (int rc = read_u32(newid.as<unsigned>() + n, h_small, 1, st)) return rc;
+    nV2 = h_small[0];
+  }
+  MC_ALLOC(oxyz, (size_t)nV2 * 12);
+  if (m.has_rgb) MC_ALLOC(orgb, (size_t)nV2 * 3);
+  if (n) k_merge_vertices<<<grid_for(n), 256, 0, st>>>(m.xyz.as<float>(), m.rgb.as<unsigned char>(), used.as<unsigned>(), newid.as<unsigned>(), n,
+                                                       oxyz.as<float>(), orgb.as<unsigned char>());
+  if (m.nF) k_merge_faces<<<grid_for(m.nF), 256, 0, st>>>(m.tri.as<unsigned>(), m.nF, ident.as<unsigned>(), newid.as<unsigned>(), otri.as<unsigned>(),
+                                                          keep.as<unsigned>());
+  m.xyz.swap(oxyz); if (m.has_rgb) m.rgb.swap(orgb); m.tri.swap(otri);
+  m.nV = nV2;
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  return SCN_OK;
+}
 
-float ms_between(cudaEvent_t a, cudaEvent_t b) { float ms = 0.f; return cudaEventElapsedTime(&ms, a, b) == cudaSuccess ? ms : 0.f; }
+int run_clean_steps(Mesh& m, const scn_mesh_clean_params& params, Scratch& s, scn_mesh_clean_report_t& rep, cudaStream_t st,
+                    unsigned* d_err, unsigned* h_small, const cudaEvent_t* ev) {
+  int rc = SCN_OK;
+  if (!(params.flags & SCN_CLEAN_SKIP_MERGE)) rc = step_merge(m, params.merge_threshold, s, rep, st, d_err, h_small);
+  if (rc) return rc;
+  SCN_CUDA_TRY(cudaEventRecord(ev[1], st));
+  if (!(params.flags & SCN_CLEAN_SKIP_DEDUP)) rc = step_dedup(m, s, rep, st);
+  if (rc) return rc;
+  SCN_CUDA_TRY(cudaEventRecord(ev[2], st));
+  if (!(params.flags & SCN_CLEAN_SKIP_PIECES)) rc = step_pieces(m, params.min_piece_vertices, params.min_piece_faces, s, rep, st, h_small);
+  if (rc) return rc;
+  SCN_CUDA_TRY(cudaEventRecord(ev[3], st));
+  SCN_CUDA_TRY(cudaEventSynchronize(ev[3]));
+  rep.merge_ms = ms_between(ev[0], ev[1]); rep.dedup_ms = ms_between(ev[1], ev[2]); rep.pieces_ms = ms_between(ev[2], ev[3]);
+  return SCN_OK;
+}
 
-}  // namespace
+}  // namespace scn::mc
+
+using namespace scn::mc;
 
 extern "C" {
 
@@ -538,16 +548,7 @@ int scn_mesh_clean(const float* xyz, const uint8_t* rgb, uint64_t nV, const uint
   SCN_CUDA_TRY(cudaEventRecord(S.ev[1], st));
   if (int rc = read_u32(err.as<unsigned>(), h_small, 1, st)) return rc;
   if (h_small[0] & ERR_INDEX) return scn::fail(SCN_ERR_ARG, "scn_mesh_clean: a face references a vertex >= %llu", (unsigned long long)nV);
-  int rc = SCN_OK;
-  if (merge) rc = step_merge(m, t, s, rep, st, err.as<unsigned>(), h_small);
-  if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[2], st));
-  if (!(params->flags & SCN_CLEAN_SKIP_DEDUP)) rc = step_dedup(m, s, rep, st);
-  if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[3], st));
-  if (!(params->flags & SCN_CLEAN_SKIP_PIECES)) rc = step_pieces(m, params->min_piece_vertices, params->min_piece_faces, s, rep, st, h_small);
-  if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[4], st));
+  if (int rc = run_clean_steps(m, *params, s, rep, st, err.as<unsigned>(), h_small, S.ev + 1)) return rc;
   float* hx = (float*)malloc(std::max<size_t>((size_t)m.nV * 12, 1));
   uint32_t* ht = (uint32_t*)malloc(std::max<size_t>((size_t)m.nF * 12, 1));
   uint8_t* hc = rgb && rgb_out ? (uint8_t*)malloc(std::max<size_t>((size_t)m.nV * 3, 1)) : nullptr;
@@ -559,8 +560,7 @@ int scn_mesh_clean(const float* xyz, const uint8_t* rgb, uint64_t nV, const uint
       cudaEventRecord(S.ev[5], st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
     return bail(scn::fail(SCN_ERR_CUDA, "scn_mesh_clean: download failed: %s", cudaGetErrorString(cudaGetLastError())));
   rep.vertices_out = m.nV; rep.faces_out = m.nF;
-  rep.upload_ms = ms_between(S.ev[0], S.ev[1]); rep.merge_ms = ms_between(S.ev[1], S.ev[2]); rep.dedup_ms = ms_between(S.ev[2], S.ev[3]);
-  rep.pieces_ms = ms_between(S.ev[3], S.ev[4]); rep.download_ms = ms_between(S.ev[4], S.ev[5]);
+  rep.upload_ms = ms_between(S.ev[0], S.ev[1]); rep.download_ms = ms_between(S.ev[4], S.ev[5]);
   rep.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   *xyz_out = hx; *tri_out = ht; if (rgb_out) *rgb_out = hc; *nV_out = m.nV; *nF_out = m.nF;
   if (report) *report = rep;
