@@ -101,13 +101,12 @@ extern "C" int scn_depth_bilateral_filter(const uint16_t* depth, uint32_t w, uin
   int ndev = 0;
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return scn::fail(SCN_ERR_CUDA, "no CUDA device");
   const size_t px = (size_t)w * h;
-  uint16_t* d_u16 = nullptr; float *d_a = nullptr, *d_b = nullptr;
-  SCN_CUDA_TRY(cudaMalloc(&d_u16, px * 2)); SCN_CUDA_TRY(cudaMalloc(&d_a, px * 4)); SCN_CUDA_TRY(cudaMalloc(&d_b, px * 4));
-  SCN_CUDA_TRY(cudaMemcpy(d_u16, depth, px * 2, cudaMemcpyHostToDevice));
+  scn::DBuf d_u16, d_a, d_b;
+  SCN_ALLOC(d_u16, px * 2); SCN_ALLOC(d_a, px * 4); SCN_ALLOC(d_b, px * 4);
+  SCN_CUDA_TRY(cudaMemcpy(d_u16.p, depth, px * 2, cudaMemcpyHostToDevice));
   BatchParams bp; bp.n = 1; bp.f[0].src = 0;
-  k_depth_to_metres_minf<<<dim3((unsigned)((px + 255) / 256), 1), 256>>>(d_u16, bp, depth_shift, px, d_a);
-  int rc = launch_filter(d_a, d_b, (int)w, (int)h, 1, sigma_d, sigma_r, nullptr);
-  if (!rc) { cudaError_t e = cudaMemcpy(out_metres, d_b, px * 4, cudaMemcpyDeviceToHost); if (e != cudaSuccess) rc = scn::fail(SCN_ERR_CUDA, "%s", cudaGetErrorString(e)); }
-  cudaFree(d_u16); cudaFree(d_a); cudaFree(d_b);
+  k_depth_to_metres_minf<<<dim3((unsigned)((px + 255) / 256), 1), 256>>>(d_u16.as<uint16_t>(), bp, depth_shift, px, d_a.as<float>());
+  int rc = launch_filter(d_a.as<float>(), d_b.as<float>(), (int)w, (int)h, 1, sigma_d, sigma_r, nullptr);
+  if (!rc) { cudaError_t e = cudaMemcpy(out_metres, d_b.p, px * 4, cudaMemcpyDeviceToHost); if (e != cudaSuccess) rc = scn::fail(SCN_ERR_CUDA, "%s", cudaGetErrorString(e)); }
   return rc;
 }

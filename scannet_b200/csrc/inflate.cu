@@ -483,29 +483,28 @@ const char* inf_msg(int rc) {
 constexpr size_t kSlice = size_t(64) << 20;
 struct InflateStage {
   int device = 0;
-  uint8_t* h[2] = {nullptr, nullptr}; cudaEvent_t ev[2] = {nullptr, nullptr};
-  cudaEvent_t tk[2] = {nullptr, nullptr};            // timing events around the kernel
-  uint8_t* d = nullptr; size_t cap = 0;
-  unsigned long long* d_off = nullptr; int* d_status = nullptr; unsigned long long* d_prod = nullptr; size_t ncap = 0;
+  scn::PinnedPtr<uint8_t> h[2]; scn::EventPtr ev[2];
+  scn::EventPtr tk[2];                               // timing events around the kernel
+  scn::DBuf d; size_t cap = 0;
+  scn::DBuf d_off, d_status, d_prod; size_t ncap = 0;   // unsigned long long, int, unsigned long long
   void release() {
-    for (int i = 0; i < 2; ++i) { if (h[i]) cudaFreeHost(h[i]); h[i] = nullptr; if (ev[i]) cudaEventDestroy(ev[i]); ev[i] = nullptr; if (tk[i]) cudaEventDestroy(tk[i]); tk[i] = nullptr; }
-    cudaFree(d); cudaFree(d_off); cudaFree(d_status); cudaFree(d_prod); d = nullptr; d_off = d_prod = nullptr; d_status = nullptr; cap = ncap = 0;
+    for (int i = 0; i < 2; ++i) { h[i].reset(); ev[i].reset(); tk[i].reset(); }
+    d.reset(); d_off.reset(); d_status.reset(); d_prod.reset(); cap = ncap = 0;
   }
   bool ensure(size_t bytes, size_t n) {
     for (int i = 0; i < 2; ++i) if (!h[i]) {
-      if (cudaHostAlloc((void**)&h[i], kSlice, cudaHostAllocDefault) != cudaSuccess || cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess ||
-          cudaEventCreate(&tk[i]) != cudaSuccess) { cudaGetLastError(); release(); return false; }
+      if (scn::create(h[i], kSlice) != cudaSuccess || scn::create(ev[i], cudaEventDisableTiming) != cudaSuccess ||
+          scn::create(tk[i]) != cudaSuccess) { cudaGetLastError(); release(); return false; }
     }
-    if (bytes > cap) {
-      cudaFree(d); d = nullptr; cap = 0;
+    if (bytes > cap) {                               // a failed allocation calls release(), which zeroes cap and ncap
       const size_t want = bytes + (bytes >> 2) + 4096;
-      if (cudaMalloc((void**)&d, want) != cudaSuccess) { cudaGetLastError(); release(); return false; }
+      if (!d.alloc(want)) { release(); return false; }
       cap = want;
     }
     if (n > ncap) {
-      cudaFree(d_off); cudaFree(d_status); cudaFree(d_prod); d_off = d_prod = nullptr; d_status = nullptr; ncap = 0;
+      d_off.reset(); d_status.reset(); d_prod.reset();
       const size_t want = n + (n >> 2) + 64;
-      if (cudaMalloc((void**)&d_off, (want + 1) * 8) != cudaSuccess || cudaMalloc((void**)&d_status, want * 4) != cudaSuccess || cudaMalloc((void**)&d_prod, want * 8) != cudaSuccess) { cudaGetLastError(); release(); return false; }
+      if (!d_off.alloc((want + 1) * 8) || !d_status.alloc(want * 4) || !d_prod.alloc(want * 8)) { release(); return false; }
       ncap = want;
     }
     return true;
@@ -548,14 +547,14 @@ int scn_inflate_batch_device(const uint8_t* const* src, const uint64_t* src_byte
   scn::StagePool<InflateStage>::Lease lease(inflate_pool());
   InflateStage& g = *lease;
   if (!g.ensure(tot + 16, n)) return scn::fail(SCN_ERR_CUDA, "scn_inflate_batch_device: allocation of %zu staging bytes failed", tot);
-  cudaError_t e = cudaMemcpyAsync(g.d_off, off.data(), ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st);
+  cudaError_t e = cudaMemcpyAsync(g.d_off.as<unsigned long long>(), off.data(), ((size_t)n + 1) * 8, cudaMemcpyHostToDevice, st);
   const unsigned nt = std::max(1u, std::min(24u, std::thread::hardware_concurrency()));     // packing is a 2-3 GB memcpy per scan: spread it
   int slot = 0; bool used[2] = {false, false};
   for (uint32_t i0 = 0; i0 < n && e == cudaSuccess;) {
     uint32_t i1 = i0; while (i1 < n && off[i1 + 1] - off[i0] <= kSlice) ++i1;               // streams [i0, i1) fit one slice
-    if (used[slot]) e = cudaEventSynchronize(g.ev[slot]);                                   // its previous upload has left the pinned slice
+    if (used[slot]) e = cudaEventSynchronize(g.ev[slot].get());                             // its previous upload has left the pinned slice
     if (e != cudaSuccess) break;
-    uint8_t* hs = g.h[slot]; const size_t base = off[i0];
+    uint8_t* hs = g.h[slot].get(); const size_t base = off[i0];
     auto fill = [&](unsigned t) {
       for (uint32_t i = i0 + t; i < i1; i += nt) {
         if (src_bytes[i]) memcpy(hs + (off[i] - base), src[i], (size_t)src_bytes[i]);
@@ -564,8 +563,8 @@ int scn_inflate_batch_device(const uint8_t* const* src, const uint64_t* src_byte
     };
     if (i1 - i0 >= 4 * nt && nt > 1) { std::vector<std::thread> pool; for (unsigned t = 1; t < nt; ++t) pool.emplace_back(fill, t); fill(0); for (auto& th : pool) th.join(); }
     else for (unsigned t = 0; t < nt; ++t) fill(t);
-    e = cudaMemcpyAsync(g.d + base, hs, (size_t)(off[i1] - base), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaEventRecord(g.ev[slot], st);
+    e = cudaMemcpyAsync(g.d.as<uint8_t>() + base, hs, (size_t)(off[i1] - base), cudaMemcpyHostToDevice, st);
+    if (e == cudaSuccess) e = cudaEventRecord(g.ev[slot].get(), st);
     used[slot] = true; slot ^= 1; i0 = i1;
   }
   std::vector<int> status(n); std::vector<unsigned long long> prod(n);
@@ -576,17 +575,17 @@ int scn_inflate_batch_device(const uint8_t* const* src, const uint64_t* src_byte
   const char* wenv = getenv("SCN_INFLATE_WINDOW");
   const bool use_ring = wenv ? !strcmp(wenv, "ring") : n <= (uint32_t)(5 * n_sm);      // at most one wave of ring streams
   if (e == cudaSuccess) {
-    cudaEventRecord(g.tk[0], st);
-    if (use_ring) k_inflate<true><<<n, 32, sizeof(InflateScratchDev), st>>>(g.d, g.d_off, (uint8_t*)d_out, (size_t)frame_bytes, (size_t)frame_bytes, n, g.d_status, g.d_prod);
-    else k_inflate<false><<<n, 32, sizeof(InflateScratch), st>>>(g.d, g.d_off, (uint8_t*)d_out, (size_t)frame_bytes, (size_t)frame_bytes, n, g.d_status, g.d_prod);
-    cudaEventRecord(g.tk[1], st);
-    e = cudaMemcpyAsync(status.data(), g.d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
+    cudaEventRecord(g.tk[0].get(), st);
+    if (use_ring) k_inflate<true><<<n, 32, sizeof(InflateScratchDev), st>>>(g.d.as<uint8_t>(), g.d_off.as<unsigned long long>(), (uint8_t*)d_out, (size_t)frame_bytes, (size_t)frame_bytes, n, g.d_status.as<int>(), g.d_prod.as<unsigned long long>());
+    else k_inflate<false><<<n, 32, sizeof(InflateScratch), st>>>(g.d.as<uint8_t>(), g.d_off.as<unsigned long long>(), (uint8_t*)d_out, (size_t)frame_bytes, (size_t)frame_bytes, n, g.d_status.as<int>(), g.d_prod.as<unsigned long long>());
+    cudaEventRecord(g.tk[1].get(), st);
+    e = cudaMemcpyAsync(status.data(), g.d_status.as<int>(), (size_t)n * 4, cudaMemcpyDeviceToHost, st);
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(prod.data(), g.d_prod, (size_t)n * 8, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(prod.data(), g.d_prod.as<unsigned long long>(), (size_t)n * 8, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) return scn::fail(SCN_ERR_CUDA, "scn_inflate_batch_device: %s", cudaGetErrorString(e));
-  { float ms = 0; if (cudaEventElapsedTime(&ms, g.tk[0], g.tk[1]) == cudaSuccess) g_last.kernel_ms = ms; g_last.pack_s = t_packed - t_call; g_last.ring = use_ring; g_last.n = n; }
+  { float ms = 0; if (cudaEventElapsedTime(&ms, g.tk[0].get(), g.tk[1].get()) == cudaSuccess) g_last.kernel_ms = ms; g_last.pack_s = t_packed - t_call; g_last.ring = use_ring; g_last.n = n; }
   for (uint32_t i = 0; i < n; ++i) {
     if (status[i] != INF_OK && status[i] != INF_OUT_FULL) return scn::fail(SCN_ERR_FORMAT, "frame %u: corrupt zlib depth stream (%s)", i, inf_msg(status[i]));
     if (prod[i] < frame_bytes) return scn::fail(SCN_ERR_FORMAT, "frame %u: depth stream holds %llu bytes, need %llu", i, prod[i], (unsigned long long)frame_bytes);

@@ -472,41 +472,41 @@ bool tail_is_plain(const uint8_t* d, size_t n, size_t pos) {
 constexpr size_t kJSlice = size_t(64) << 20;
 struct JpegStage {
   int device = 0;
-  uint8_t* h[2] = {nullptr, nullptr}; cudaEvent_t ev[2] = {nullptr, nullptr};
-  cudaEvent_t tk[3] = {nullptr, nullptr, nullptr};   // timing events: before the entropy kernel, between, after the colour kernel
-  uint8_t* d_in = nullptr; size_t in_cap = 0;
-  uint8_t* d_planes = nullptr; size_t planes_cap = 0;
-  FrameDesc* d_fd = nullptr; int* d_status = nullptr; unsigned* d_end = nullptr; size_t ncap = 0;
-  TableSet* d_sets = nullptr; size_t sets_cap = 0;
+  scn::PinnedPtr<uint8_t> h[2]; scn::EventPtr ev[2];
+  scn::EventPtr tk[3];                               // timing events: before the entropy kernel, between, after the colour kernel
+  scn::DBuf d_in; size_t in_cap = 0;                 // uint8_t
+  scn::DBuf d_planes; size_t planes_cap = 0;         // uint8_t
+  scn::DBuf d_fd, d_status, d_end; size_t ncap = 0;  // FrameDesc, int, unsigned
+  scn::DBuf d_sets; size_t sets_cap = 0;             // TableSet
   bool ensure(size_t in_bytes, size_t plane_bytes, size_t n, size_t nsets) {
     for (int i = 0; i < 2; ++i) if (!h[i]) {
-      if (cudaHostAlloc((void**)&h[i], kJSlice, cudaHostAllocDefault) != cudaSuccess || cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return false; }
+      if (scn::create(h[i], kJSlice) != cudaSuccess || scn::create(ev[i], cudaEventDisableTiming) != cudaSuccess) { cudaGetLastError(); return false; }
     }
-    for (int i = 0; i < 3; ++i) if (!tk[i] && cudaEventCreate(&tk[i]) != cudaSuccess) { cudaGetLastError(); return false; }
-    auto grow = [](void** p, size_t* cap, size_t want) {
+    for (int i = 0; i < 3; ++i) if (!tk[i] && scn::create(tk[i]) != cudaSuccess) { cudaGetLastError(); return false; }
+    auto grow = [](scn::DBuf& b, size_t* cap, size_t want) {
       if (want <= *cap) return true;
-      cudaFree(*p); *p = nullptr; *cap = 0;
+      *cap = 0;
       const size_t w = want + (want >> 2) + 4096;
-      if (cudaMalloc(p, w) != cudaSuccess) { cudaGetLastError(); return false; }
+      if (!b.alloc(w)) return false;
       *cap = w; return true;
     };
-    if (!grow((void**)&d_in, &in_cap, in_bytes) || !grow((void**)&d_planes, &planes_cap, plane_bytes)) return false;
+    if (!grow(d_in, &in_cap, in_bytes) || !grow(d_planes, &planes_cap, plane_bytes)) return false;
     if (n > ncap) {
-      cudaFree(d_fd); cudaFree(d_status); cudaFree(d_end); d_fd = nullptr; d_status = nullptr; d_end = nullptr; ncap = 0;
+      d_fd.reset(); d_status.reset(); d_end.reset(); ncap = 0;
       const size_t w = n + (n >> 2) + 64;
-      if (cudaMalloc((void**)&d_fd, w * sizeof(FrameDesc)) != cudaSuccess || cudaMalloc((void**)&d_status, w * 4) != cudaSuccess || cudaMalloc((void**)&d_end, w * 4) != cudaSuccess) { cudaGetLastError(); return false; }
+      if (!d_fd.alloc(w * sizeof(FrameDesc)) || !d_status.alloc(w * 4) || !d_end.alloc(w * 4)) return false;
       ncap = w;
     }
     size_t sc = sets_cap * sizeof(TableSet);
-    if (!grow((void**)&d_sets, &sc, nsets * sizeof(TableSet))) return false;
+    if (!grow(d_sets, &sc, nsets * sizeof(TableSet))) return false;
     sets_cap = sc / sizeof(TableSet);
     return true;
   }
   void release() {
-    for (int i = 0; i < 2; ++i) { if (h[i]) cudaFreeHost(h[i]); h[i] = nullptr; if (ev[i]) cudaEventDestroy(ev[i]); ev[i] = nullptr; }
-    for (int i = 0; i < 3; ++i) { if (tk[i]) cudaEventDestroy(tk[i]); tk[i] = nullptr; }
-    cudaFree(d_in); cudaFree(d_planes); cudaFree(d_fd); cudaFree(d_status); cudaFree(d_end); cudaFree(d_sets);
-    d_in = d_planes = nullptr; d_fd = nullptr; d_status = nullptr; d_end = nullptr; d_sets = nullptr; in_cap = planes_cap = ncap = sets_cap = 0;
+    for (int i = 0; i < 2; ++i) { h[i].reset(); ev[i].reset(); }
+    for (int i = 0; i < 3; ++i) tk[i].reset();
+    d_in.reset(); d_planes.reset(); d_fd.reset(); d_status.reset(); d_end.reset(); d_sets.reset();
+    in_cap = planes_cap = ncap = sets_cap = 0;
   }
 };
 scn::StagePool<JpegStage>& jpeg_pool() { static auto* p = new scn::StagePool<JpegStage>(); return *p; }
@@ -562,17 +562,17 @@ int scn_jpeg_decode_batch_device(const uint8_t* const* src, const uint64_t* src_
   if (!g.ensure(in_total + 16, plane_stride * n + 16, n, std::max<size_t>(1, sets.size()))) return scn::fail(SCN_ERR_CUDA, "scn_jpeg_decode_batch_device: device staging allocation failed");
   std::vector<FrameDesc> fd(n);
   for (uint32_t i = 0; i < n; ++i) fd[i] = P[i].d;
-  cudaError_t e = cudaMemcpyAsync(g.d_fd, fd.data(), n * sizeof(FrameDesc), cudaMemcpyHostToDevice, st);
-  if (e == cudaSuccess && !sets.empty()) e = cudaMemcpyAsync(g.d_sets, sets.data(), sets.size() * sizeof(TableSet), cudaMemcpyHostToDevice, st);
+  cudaError_t e = cudaMemcpyAsync(g.d_fd.as<FrameDesc>(), fd.data(), n * sizeof(FrameDesc), cudaMemcpyHostToDevice, st);
+  if (e == cudaSuccess && !sets.empty()) e = cudaMemcpyAsync(g.d_sets.as<TableSet>(), sets.data(), sets.size() * sizeof(TableSet), cudaMemcpyHostToDevice, st);
   // 2. pack + upload the supported payloads through the two pinned slices
   {
     const unsigned nt = std::max(1u, std::min(24u, std::thread::hardware_concurrency()));     // packing is a 2-3 GB memcpy per scan: spread it
     int slot = 0; bool used[2] = {false, false};
     for (uint32_t i0 = 0; i0 < n && e == cudaSuccess;) {
       uint32_t i1 = i0; while (i1 < n && off[i1 + 1] - off[i0] <= kJSlice) ++i1;
-      if (used[slot]) e = cudaEventSynchronize(g.ev[slot]);
+      if (used[slot]) e = cudaEventSynchronize(g.ev[slot].get());
       if (e != cudaSuccess) break;
-      uint8_t* hs = g.h[slot]; const size_t base = off[i0];
+      uint8_t* hs = g.h[slot].get(); const size_t base = off[i0];
       auto fill = [&](unsigned t) {
         for (uint32_t i = i0 + t; i < i1; i += nt) if (P[i].ok) {
           memcpy(hs + (off[i] - base), src[i], (size_t)src_bytes[i]);
@@ -581,8 +581,8 @@ int scn_jpeg_decode_batch_device(const uint8_t* const* src, const uint64_t* src_
       };
       if (i1 - i0 >= 4 * nt && nt > 1) { std::vector<std::thread> pool; for (unsigned t = 1; t < nt; ++t) pool.emplace_back(fill, t); fill(0); for (auto& th : pool) th.join(); }
       else for (unsigned t = 0; t < nt; ++t) fill(t);
-      if (off[i1] > base) e = cudaMemcpyAsync(g.d_in + base, hs, (size_t)(off[i1] - base), cudaMemcpyHostToDevice, st);
-      if (e == cudaSuccess) e = cudaEventRecord(g.ev[slot], st);
+      if (off[i1] > base) e = cudaMemcpyAsync(g.d_in.as<uint8_t>() + base, hs, (size_t)(off[i1] - base), cudaMemcpyHostToDevice, st);
+      if (e == cudaSuccess) e = cudaEventRecord(g.ev[slot].get(), st);
       used[slot] = true; slot ^= 1; i0 = i1;
     }
   }
@@ -590,12 +590,12 @@ int scn_jpeg_decode_batch_device(const uint8_t* const* src, const uint64_t* src_
   std::vector<int> status(n, JST_UNSUPPORTED); std::vector<unsigned> endp(n, 0);
   const double t_packed = std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count();
   if (e == cudaSuccess) {
-    cudaEventRecord(g.tk[0], st);
-    k_jpeg_entropy_idct<<<n, 32, 0, st>>>(g.d_in, g.d_fd, g.d_sets, g.d_planes, plane_stride, g.d_status, g.d_end);
-    cudaEventRecord(g.tk[1], st);
-    e = cudaMemcpyAsync(status.data(), g.d_status, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
+    cudaEventRecord(g.tk[0].get(), st);
+    k_jpeg_entropy_idct<<<n, 32, 0, st>>>(g.d_in.as<uint8_t>(), g.d_fd.as<FrameDesc>(), g.d_sets.as<TableSet>(), g.d_planes.as<uint8_t>(), plane_stride, g.d_status.as<int>(), g.d_end.as<unsigned>());
+    cudaEventRecord(g.tk[1].get(), st);
+    e = cudaMemcpyAsync(status.data(), g.d_status.as<int>(), (size_t)n * 4, cudaMemcpyDeviceToHost, st);
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(endp.data(), g.d_end, (size_t)n * 4, cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(endp.data(), g.d_end.as<unsigned>(), (size_t)n * 4, cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
   // multi-scan files: what follows the scan must be padding / EOI, else the host decoder takes the frame
   std::vector<uint32_t> redo;
@@ -605,19 +605,19 @@ int scn_jpeg_decode_batch_device(const uint8_t* const* src, const uint64_t* src_
       if (status[i] == JST_OK && !tail_is_plain(src[i], (size_t)src_bytes[i], endp[i])) { status[i] = JST_UNSUPPORTED; changed = true; }
       if (status[i] != JST_OK) redo.push_back(i);
     }
-    if (changed) e = cudaMemcpyAsync(g.d_status, status.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st);
+    if (changed) e = cudaMemcpyAsync(g.d_status.as<int>(), status.data(), (size_t)n * 4, cudaMemcpyHostToDevice, st);
   }
   if (e == cudaSuccess) {
     if (!d_lut && out_px % 4 == 0 && (reinterpret_cast<uintptr_t>(d_out) & 3) == 0)
-      k_jpeg_color4<<<dim3((out_px + 1023) / 1024, n), 256, 0, st>>>(g.d_fd, g.d_planes, plane_stride, g.d_status, out_px, (unsigned char*)d_out);
+      k_jpeg_color4<<<dim3((out_px + 1023) / 1024, n), 256, 0, st>>>(g.d_fd.as<FrameDesc>(), g.d_planes.as<uint8_t>(), plane_stride, g.d_status.as<int>(), out_px, (unsigned char*)d_out);
     else
-      k_jpeg_color<<<dim3((out_px + 255) / 256, n), 256, 0, st>>>(g.d_fd, g.d_planes, plane_stride, g.d_status, d_lut, out_px, (unsigned char*)d_out);
-    cudaEventRecord(g.tk[2], st);
+      k_jpeg_color<<<dim3((out_px + 255) / 256, n), 256, 0, st>>>(g.d_fd.as<FrameDesc>(), g.d_planes.as<uint8_t>(), plane_stride, g.d_status.as<int>(), d_lut, out_px, (unsigned char*)d_out);
+    cudaEventRecord(g.tk[2].get(), st);
     e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
     float ms = 0;
-    if (e == cudaSuccess && cudaEventElapsedTime(&ms, g.tk[0], g.tk[1]) == cudaSuccess) g_jlast.entropy_ms = ms;
-    if (e == cudaSuccess && cudaEventElapsedTime(&ms, g.tk[1], g.tk[2]) == cudaSuccess) g_jlast.color_ms = ms;
+    if (e == cudaSuccess && cudaEventElapsedTime(&ms, g.tk[0].get(), g.tk[1].get()) == cudaSuccess) g_jlast.entropy_ms = ms;
+    if (e == cudaSuccess && cudaEventElapsedTime(&ms, g.tk[1].get(), g.tk[2].get()) == cudaSuccess) g_jlast.color_ms = ms;
     g_jlast.host_s = t_packed - t_call;
   }
   if (e != cudaSuccess) return scn::fail(SCN_ERR_CUDA, "scn_jpeg_decode_batch_device: %s", cudaGetErrorString(e));

@@ -187,70 +187,67 @@ __global__ void k_mc_compact(const float* __restrict__ vpos, const uint8_t* __re
   for (int q = 0; q < 3; ++q) { opos[3 * k + q] = vpos[3 * i + q]; orgb[3 * k + q] = vrgb[3 * i + q]; }
 }
 
-struct Buf { void* p = nullptr; ~Buf() { if (p) cudaFree(p); } int alloc(size_t n) { return cudaMalloc(&p, n ? n : 16) == cudaSuccess ? 0 : -1; } template <class T> T* as() { return (T*)p; } };
-
 }  // namespace
-
-#define MCK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) return scn::fail(SCN_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); } while (0)
 
 extern "C" int scn_tsdf_extract_mesh(scn_tsdf* t, float** xyz, uint8_t** rgb, uint32_t** tri, uint64_t* n_verts, uint64_t* n_faces) {
   if (!t || !xyz || !tri || !n_verts || !n_faces) return scn::fail(SCN_ERR_ARG, "null argument");
-  MCK(cudaSetDevice(t->device));
-  MCK(cudaStreamSynchronize(t->stream));
+  SCN_CUDA_TRY(cudaSetDevice(t->device));
+  SCN_CUDA_TRY(cudaStreamSynchronize(t->stream));
   cudaStream_t st = t->stream;
   unsigned long long cnt[C_COUNT];
-  MCK(cudaMemcpy(cnt, t->tb.counters, sizeof(cnt), cudaMemcpyDeviceToHost));
+  SCN_CUDA_TRY(cudaMemcpy(cnt, t->tb.counters, sizeof(cnt), cudaMemcpyDeviceToHost));
   const size_t N = (size_t)std::min<unsigned long long>(cnt[C_HEAP], t->tb.max_blocks);
   *n_verts = *n_faces = 0; *xyz = nullptr; *tri = nullptr; if (rgb) *rgb = nullptr;
   if (N == 0) { *xyz = (float*)malloc(16); *tri = (uint32_t*)malloc(16); if (rgb) *rgb = (uint8_t*)malloc(16); return SCN_OK; }
   // deterministic block order: ascending packed key
   std::vector<unsigned long long> keys(N);
-  MCK(cudaMemcpy(keys.data(), t->tb.block_keys, N * 8, cudaMemcpyDeviceToHost));
+  SCN_CUDA_TRY(cudaMemcpy(keys.data(), t->tb.block_keys, N * 8, cudaMemcpyDeviceToHost));
   std::vector<unsigned> order(N), inv(N);
   std::iota(order.begin(), order.end(), 0u);
   std::sort(order.begin(), order.end(), [&](unsigned a, unsigned b) { return keys[a] < keys[b]; });
   for (size_t j = 0; j < N; ++j) inv[order[j]] = (unsigned)j;
   McTable tab; build_mc_table(tab);
   const size_t NV = N * 512;
-  Buf dOrder, dInv, dTab, dFl, dVc, dTc, dVb, dTb, dScr;
-  if (dOrder.alloc(N * 4) || dInv.alloc(N * 4) || dTab.alloc(sizeof(McTable)) || dFl.alloc(NV) || dVc.alloc(NV * 4) || dTc.alloc(NV * 4) ||
-      dVb.alloc((NV + 1) * 4) || dTb.alloc((NV + 1) * 4) || dScr.alloc(scn::scan_scratch_elems(NV) * 4))
+  scn::DBuf dOrder, dInv, dTab, dFl, dVc, dTc, dVb, dTb, dScr;
+  if (!dOrder.alloc(N * 4) || !dInv.alloc(N * 4) || !dTab.alloc(sizeof(McTable)) || !dFl.alloc(NV) || !dVc.alloc(NV * 4) || !dTc.alloc(NV * 4) ||
+      !dVb.alloc((NV + 1) * 4) || !dTb.alloc((NV + 1) * 4) || !dScr.alloc(scn::scan_scratch_elems(NV) * 4))
     return scn::fail(SCN_ERR_CUDA, "cudaMalloc (marching cubes workspace, %zu blocks)", N);
-  MCK(cudaMemcpyAsync(dOrder.p, order.data(), N * 4, cudaMemcpyHostToDevice, st));
-  MCK(cudaMemcpyAsync(dInv.p, inv.data(), N * 4, cudaMemcpyHostToDevice, st));
-  MCK(cudaMemcpyAsync(dTab.p, &tab, sizeof(tab), cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dOrder.p, order.data(), N * 4, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dInv.p, inv.data(), N * 4, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dTab.p, &tab, sizeof(tab), cudaMemcpyHostToDevice, st));
   McCtx c; c.tb = t->tb; c.order = dOrder.as<unsigned>(); c.inv_order = dInv.as<unsigned>(); c.n_blocks = (unsigned)N;
   { volatile float th = t->mc_thresh_factor * t->vp.vs; c.thr = th; } c.vs = t->vp.vs;
   k_mc_count<<<(unsigned)N, 512, 0, st>>>(c, dTab.as<McTable>(), dFl.as<uint8_t>(), dVc.as<unsigned>(), dTc.as<unsigned>());
   scn::exclusive_scan_u32(dVc.as<unsigned>(), dVb.as<unsigned>(), NV, dScr.as<unsigned>(), st);
   scn::exclusive_scan_u32(dTc.as<unsigned>(), dTb.as<unsigned>(), NV, dScr.as<unsigned>(), st);
   unsigned nV0 = 0, nT = 0;
-  MCK(cudaMemcpyAsync(&nV0, dVb.as<unsigned>() + NV, 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaMemcpyAsync(&nT, dTb.as<unsigned>() + NV, 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaStreamSynchronize(st));
-  Buf dPos, dRgb, dTri, dUsed, dNew, dPos2, dRgb2;
-  if (dPos.alloc((size_t)nV0 * 12) || dRgb.alloc((size_t)nV0 * 3) || dTri.alloc((size_t)nT * 12) || dUsed.alloc((size_t)nV0 * 4) || dNew.alloc(((size_t)nV0 + 1) * 4))
+  SCN_CUDA_TRY(cudaMemcpyAsync(&nV0, dVb.as<unsigned>() + NV, 4, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(&nT, dTb.as<unsigned>() + NV, 4, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  scn::DBuf dPos, dRgb, dTri, dUsed, dNew, dPos2, dRgb2;
+  if (!dPos.alloc((size_t)nV0 * 12) || !dRgb.alloc((size_t)nV0 * 3) || !dTri.alloc((size_t)nT * 12) || !dUsed.alloc((size_t)nV0 * 4) || !dNew.alloc(((size_t)nV0 + 1) * 4))
     return scn::fail(SCN_ERR_CUDA, "cudaMalloc (mesh buffers: %u vertices, %u triangles)", nV0, nT);
-  MCK(cudaMemsetAsync(dUsed.p, 0, (size_t)nV0 * 4, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(dUsed.p, 0, (size_t)nV0 * 4, st));
   k_mc_emit<<<(unsigned)N, 512, 0, st>>>(c, dTab.as<McTable>(), dFl.as<uint8_t>(), dVb.as<unsigned>(), dTb.as<unsigned>(), dPos.as<float>(),
                                           dRgb.as<uint8_t>(), dTri.as<unsigned>(), dUsed.as<unsigned>());
-  Buf dScr2; if (dScr2.alloc(scn::scan_scratch_elems(nV0) * 4)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc");
+  scn::DBuf dScr2; if (!dScr2.alloc(scn::scan_scratch_elems(nV0) * 4)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc");
   scn::exclusive_scan_u32(dUsed.as<unsigned>(), dNew.as<unsigned>(), nV0, dScr2.as<unsigned>(), st);
   unsigned nV = 0;
-  MCK(cudaMemcpyAsync(&nV, dNew.as<unsigned>() + nV0, 4, cudaMemcpyDeviceToHost, st));
-  MCK(cudaStreamSynchronize(st));
-  if (dPos2.alloc((size_t)nV * 12) || dRgb2.alloc((size_t)nV * 3)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc");
+  SCN_CUDA_TRY(cudaMemcpyAsync(&nV, dNew.as<unsigned>() + nV0, 4, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  if (!dPos2.alloc((size_t)nV * 12) || !dRgb2.alloc((size_t)nV * 3)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc");
   if (nT) k_mc_remap<<<(unsigned)(((size_t)nT * 3 + 255) / 256), 256, 0, st>>>(dTri.as<unsigned>(), (size_t)nT * 3, dNew.as<unsigned>());
   if (nV0) k_mc_compact<<<(unsigned)(((size_t)nV0 + 255) / 256), 256, 0, st>>>(dPos.as<float>(), dRgb.as<uint8_t>(), dUsed.as<unsigned>(), dNew.as<unsigned>(), nV0,
                                                                                 dPos2.as<float>(), dRgb2.as<uint8_t>());
-  MCK(cudaGetLastError());
-  *xyz = (float*)malloc(std::max<size_t>(16, (size_t)nV * 12)); *tri = (uint32_t*)malloc(std::max<size_t>(16, (size_t)nT * 12));
-  uint8_t* hrgb = (uint8_t*)malloc(std::max<size_t>(16, (size_t)nV * 3));
-  if (!*xyz || !*tri || !hrgb) return scn::fail(SCN_ERR_ARG, "out of host memory");
-  MCK(cudaMemcpy(*xyz, dPos2.p, (size_t)nV * 12, cudaMemcpyDeviceToHost));
-  MCK(cudaMemcpy(hrgb, dRgb2.p, (size_t)nV * 3, cudaMemcpyDeviceToHost));
-  MCK(cudaMemcpy(*tri, dTri.p, (size_t)nT * 12, cudaMemcpyDeviceToHost));
-  if (rgb) *rgb = hrgb; else free(hrgb);
+  SCN_CUDA_TRY(cudaGetLastError());
+  scn::MallocPtr<float> hxyz((float*)malloc(std::max<size_t>(16, (size_t)nV * 12)));
+  scn::MallocPtr<uint32_t> htri((uint32_t*)malloc(std::max<size_t>(16, (size_t)nT * 12)));
+  scn::MallocPtr<uint8_t> hrgb((uint8_t*)malloc(std::max<size_t>(16, (size_t)nV * 3)));
+  if (!hxyz || !htri || !hrgb) return scn::fail(SCN_ERR_ARG, "out of host memory");
+  SCN_CUDA_TRY(cudaMemcpy(hxyz.get(), dPos2.p, (size_t)nV * 12, cudaMemcpyDeviceToHost));
+  SCN_CUDA_TRY(cudaMemcpy(hrgb.get(), dRgb2.p, (size_t)nV * 3, cudaMemcpyDeviceToHost));
+  SCN_CUDA_TRY(cudaMemcpy(htri.get(), dTri.p, (size_t)nT * 12, cudaMemcpyDeviceToHost));
+  *xyz = hxyz.release(); *tri = htri.release(); if (rgb) *rgb = hrgb.release();
   *n_verts = nV; *n_faces = nT;
   t->launches += 8;
   return SCN_OK;

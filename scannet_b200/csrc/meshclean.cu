@@ -29,11 +29,6 @@
 
 namespace scn::mc {
 
-using scn::bits_for;
-using scn::k_iota;
-using scn::radix_sort_pairs;
-using scn::rs_hist_elems;
-
 enum : unsigned { ERR_INDEX = 1u, ERR_CELL = 2u };
 __device__ __forceinline__ size_t tid() { return blockIdx.x * (size_t)blockDim.x + threadIdx.x; }
 
@@ -300,15 +295,33 @@ int read_u32(const unsigned* d, unsigned* h, size_t n, cudaStream_t st) {
   return SCN_OK;
 }
 
-// sorts `val` (initially any permutation) stably by key, leaving the result in (k0,v0) or (k1,v1); returns the value array
-unsigned* sort_pass(Scratch& s, unsigned*& vals, size_t n, int bits, cudaStream_t st) {
-  unsigned* k0 = s.k0.as<unsigned>(); unsigned* k1 = s.k1.as<unsigned>();
-  unsigned* v0 = s.v0.as<unsigned>(); unsigned* v1 = s.v1.as<unsigned>();
-  // keys are always staged in k0 and values in `vals` (== v0 or v1)
-  if (vals != v0) { cudaMemcpyAsync(v0, vals, n * 4, cudaMemcpyDeviceToDevice, st); }
-  const int w = radix_sort_pairs(k0, v0, k1, v1, n, bits, s.hist.as<unsigned>(), s.scr.as<unsigned>(), st);
-  vals = w ? v1 : v0;
-  return vals;
+int upload_mesh(Mesh& m, const float* xyz, const uint8_t* rgb, uint64_t nV, const uint32_t* tri, uint64_t nF, PinnedPtr<unsigned>& h_small,
+                DBuf& err, cudaEvent_t start, cudaStream_t st) {
+  SCN_CUDA_TRY(create(h_small, 16));
+  m.nV = (unsigned)nV; m.nF = (unsigned)nF; m.has_rgb = rgb != nullptr;
+  SCN_ALLOC(m.xyz, nV * 12); SCN_ALLOC(m.tri, nF * 12); SCN_ALLOC(err, 4);
+  if (m.has_rgb) SCN_ALLOC(m.rgb, nV * 3);
+  SCN_CUDA_TRY(cudaEventRecord(start, st));
+  if (nV) SCN_CUDA_TRY(cudaMemcpyAsync(m.xyz.p, xyz, nV * 12, cudaMemcpyHostToDevice, st));
+  if (nV && rgb) SCN_CUDA_TRY(cudaMemcpyAsync(m.rgb.p, rgb, nV * 3, cudaMemcpyHostToDevice, st));
+  if (nF) SCN_CUDA_TRY(cudaMemcpyAsync(m.tri.p, tri, nF * 12, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, st));
+  return SCN_OK;
+}
+
+int download_mesh(const Mesh& m, float** xyz, uint8_t** rgb, uint32_t** tri, cudaEvent_t done, cudaStream_t st, const char* who) {
+  const bool want_rgb = m.has_rgb && rgb;
+  MallocPtr<float> hx((float*)malloc(std::max<size_t>((size_t)m.nV * 12, 1)));
+  MallocPtr<uint32_t> ht((uint32_t*)malloc(std::max<size_t>((size_t)m.nF * 12, 1)));
+  MallocPtr<uint8_t> hc(want_rgb ? (uint8_t*)malloc(std::max<size_t>((size_t)m.nV * 3, 1)) : nullptr);
+  if (!hx || !ht || (want_rgb && !hc)) return scn::fail(SCN_ERR_ARG, "%s: out of host memory", who);
+  if ((m.nV && cudaMemcpyAsync(hx.get(), m.xyz.p, (size_t)m.nV * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
+      (m.nF && cudaMemcpyAsync(ht.get(), m.tri.p, (size_t)m.nF * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
+      (hc && m.nV && cudaMemcpyAsync(hc.get(), m.rgb.p, (size_t)m.nV * 3, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
+      cudaEventRecord(done, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
+    return scn::fail(SCN_ERR_CUDA, "%s: download failed: %s", who, cudaGetErrorString(cudaGetLastError()));
+  *xyz = hx.release(); *tri = ht.release(); if (rgb) *rgb = hc.release();
+  return SCN_OK;
 }
 
 int step_merge(Mesh& m, float t, Scratch& s, scn_mesh_clean_report_t& rep, cudaStream_t st, unsigned* d_err, unsigned* h_small) {
@@ -317,7 +330,7 @@ int step_merge(Mesh& m, float t, Scratch& s, scn_mesh_clean_report_t& rep, cudaS
   const float inv = 1.0f / t, tsq = t * t;
   DBuf cell, order, head, hidx, ucell, ustart, cellidx, nb, par, size, stats, target, rep_flag, newid, oxyz, orgb, otri, keep, fpos;
   if (int rc = s.ensure(n, std::max<size_t>(n, m.nF) + 1)) return rc;
-  MC_ALLOC(cell, (size_t)n * 12); MC_ALLOC(order, (size_t)n * 4);
+  SCN_ALLOC(cell, (size_t)n * 12); SCN_ALLOC(order, (size_t)n * 4);
   unsigned* k0 = s.k0.as<unsigned>();
   unsigned* vals = s.v0.as<unsigned>();
   k_cells<<<grid_for(n), 256, 0, st>>>(m.xyz.as<float>(), n, inv, cell.as<int>(), k0, vals, d_err);
@@ -332,15 +345,15 @@ int step_merge(Mesh& m, float t, Scratch& s, scn_mesh_clean_report_t& rep, cudaS
   k_gather_axis<<<grid_for(n), 256, 0, st>>>(cell.as<int>(), 2, vals, n, k0);
   sort_pass(s, vals, n, 32, st);
   SCN_CUDA_TRY(cudaMemcpyAsync(order.p, vals, (size_t)n * 4, cudaMemcpyDeviceToDevice, st));
-  MC_ALLOC(head, (size_t)n * 4); MC_ALLOC(hidx, ((size_t)n + 1) * 4); MC_ALLOC(ucell, (size_t)n * 12); MC_ALLOC(ustart, ((size_t)n + 1) * 4);
-  MC_ALLOC(cellidx, (size_t)n * 4); MC_ALLOC(nb, (size_t)n * 27 * 4);
+  SCN_ALLOC(head, (size_t)n * 4); SCN_ALLOC(hidx, ((size_t)n + 1) * 4); SCN_ALLOC(ucell, (size_t)n * 12); SCN_ALLOC(ustart, ((size_t)n + 1) * 4);
+  SCN_ALLOC(cellidx, (size_t)n * 4); SCN_ALLOC(nb, (size_t)n * 27 * 4);
   k_cell_heads<<<grid_for(n), 256, 0, st>>>(cell.as<int>(), order.as<unsigned>(), n, head.as<unsigned>());
   scn::exclusive_scan_u32(head.as<unsigned>(), hidx.as<unsigned>(), n, s.scr.as<unsigned>(), st);
   k_cell_table<<<grid_for(n), 256, 0, st>>>(cell.as<int>(), order.as<unsigned>(), head.as<unsigned>(), hidx.as<unsigned>(), n,
                                             ucell.as<int>(), ustart.as<unsigned>(), cellidx.as<unsigned>());
   k_cell_neighbours<<<grid_for(n), 256, 0, st>>>(ucell.as<int>(), hidx.as<unsigned>() + n, nb.as<int>());
   // proximity components
-  MC_ALLOC(par, (size_t)n * 4); MC_ALLOC(size, (size_t)n * 4); MC_ALLOC(stats, 8);
+  SCN_ALLOC(par, (size_t)n * 4); SCN_ALLOC(size, (size_t)n * 4); SCN_ALLOC(stats, 8);
   k_iota<<<grid_for(n), 256, 0, st>>>(par.as<unsigned>(), n);
   k_merge_union<<<grid_for(n), 256, 0, st>>>(m.xyz.as<float>(), cellidx.as<unsigned>(), nb.as<int>(), ustart.as<unsigned>(), order.as<unsigned>(),
                                              n, tsq, par.as<unsigned>());
@@ -352,7 +365,7 @@ int step_merge(Mesh& m, float t, Scratch& s, scn_mesh_clean_report_t& rep, cudaS
   k_iota<<<grid_for(n), 256, 0, st>>>(s.v0.as<unsigned>(), n);
   vals = s.v0.as<unsigned>();
   unsigned* skeys = sort_pass(s, vals, n, bits_for(n - 1), st) == s.v0.as<unsigned>() ? s.k0.as<unsigned>() : s.k1.as<unsigned>();
-  MC_ALLOC(target, (size_t)n * 4); MC_ALLOC(rep_flag, (size_t)n * 4); MC_ALLOC(newid, ((size_t)n + 1) * 4);
+  SCN_ALLOC(target, (size_t)n * 4); SCN_ALLOC(rep_flag, (size_t)n * 4); SCN_ALLOC(newid, ((size_t)n + 1) * 4);
   k_merge_replay<<<grid_for(n), 256, 0, st>>>(skeys, vals, n, m.xyz.as<float>(), cellidx.as<unsigned>(), nb.as<int>(), ustart.as<unsigned>(),
                                               order.as<unsigned>(), tsq, rep_flag.as<unsigned>(), target.as<unsigned>());
   scn::exclusive_scan_u32(rep_flag.as<unsigned>(), newid.as<unsigned>(), n, s.scr.as<unsigned>(), st);
@@ -361,13 +374,13 @@ int step_merge(Mesh& m, float t, Scratch& s, scn_mesh_clean_report_t& rep, cudaS
   if (int rc = read_u32(stats.as<unsigned>(), h_small, 2, st)) return rc;
   rep.largest_merge_component = h_small[0]; rep.merge_components = h_small[1];
   rep.vertices_merged = n - nV2;
-  MC_ALLOC(oxyz, (size_t)nV2 * 12);
-  if (m.has_rgb) MC_ALLOC(orgb, (size_t)nV2 * 3);
+  SCN_ALLOC(oxyz, (size_t)nV2 * 12);
+  if (m.has_rgb) SCN_ALLOC(orgb, (size_t)nV2 * 3);
   k_merge_vertices<<<grid_for(n), 256, 0, st>>>(m.xyz.as<float>(), m.rgb.as<unsigned char>(), rep_flag.as<unsigned>(), newid.as<unsigned>(), n,
                                                 oxyz.as<float>(), orgb.as<unsigned char>());
   unsigned nF2 = 0;
   if (m.nF) {
-    MC_ALLOC(otri, (size_t)m.nF * 12); MC_ALLOC(keep, (size_t)m.nF * 4); MC_ALLOC(fpos, ((size_t)m.nF + 1) * 4);
+    SCN_ALLOC(otri, (size_t)m.nF * 12); SCN_ALLOC(keep, (size_t)m.nF * 4); SCN_ALLOC(fpos, ((size_t)m.nF + 1) * 4);
     k_merge_faces<<<grid_for(m.nF), 256, 0, st>>>(m.tri.as<unsigned>(), m.nF, target.as<unsigned>(), newid.as<unsigned>(), otri.as<unsigned>(), keep.as<unsigned>());
     scn::exclusive_scan_u32(keep.as<unsigned>(), fpos.as<unsigned>(), m.nF, s.scr.as<unsigned>(), st);
     if (int rc = read_u32(fpos.as<unsigned>() + m.nF, &nF2, 1, st)) return rc;
@@ -385,7 +398,7 @@ int step_dedup(Mesh& m, Scratch& s, scn_mesh_clean_report_t& rep, cudaStream_t s
   if (nF == 0) return SCN_OK;
   if (int rc = s.ensure(nF, (size_t)nF + 1)) return rc;
   DBuf keep, fpos, otri;
-  MC_ALLOC(keep, (size_t)nF * 4); MC_ALLOC(fpos, ((size_t)nF + 1) * 4); MC_ALLOC(otri, (size_t)nF * 12);
+  SCN_ALLOC(keep, (size_t)nF * 4); SCN_ALLOC(fpos, ((size_t)nF + 1) * 4); SCN_ALLOC(otri, (size_t)nF * 12);
   const int bits = bits_for(m.nV ? m.nV - 1 : 0);
   unsigned* k0 = s.k0.as<unsigned>();
   unsigned* vals = s.v0.as<unsigned>();
@@ -410,7 +423,7 @@ int step_pieces(Mesh& m, unsigned min_v, unsigned min_f, Scratch& s, scn_mesh_cl
   const unsigned n = m.nV, nF = m.nF;
   if (int rc = s.ensure(std::max(n, nF), 3 * (size_t)nF + 1)) return rc;
   DBuf par, root, vcount, fcount, stats, keep, fpos, ktri, first, flag, cpos, otri, oxyz, orgb;
-  MC_ALLOC(par, (size_t)n * 4); MC_ALLOC(root, (size_t)n * 4); MC_ALLOC(vcount, (size_t)n * 4); MC_ALLOC(fcount, (size_t)n * 4); MC_ALLOC(stats, 12);
+  SCN_ALLOC(par, (size_t)n * 4); SCN_ALLOC(root, (size_t)n * 4); SCN_ALLOC(vcount, (size_t)n * 4); SCN_ALLOC(fcount, (size_t)n * 4); SCN_ALLOC(stats, 12);
   SCN_CUDA_TRY(cudaMemsetAsync(stats.p, 0, 12, st));
   unsigned nF2 = 0, nV2 = 0;
   if (n) {
@@ -423,7 +436,7 @@ int step_pieces(Mesh& m, unsigned min_v, unsigned min_f, Scratch& s, scn_mesh_cl
     k_piece_stats<<<grid_for(n), 256, 0, st>>>(root.as<unsigned>(), vcount.as<unsigned>(), fcount.as<unsigned>(), n, min_v, min_f, stats.as<unsigned>());
   }
   if (nF) {
-    MC_ALLOC(keep, (size_t)nF * 4); MC_ALLOC(fpos, ((size_t)nF + 1) * 4); MC_ALLOC(ktri, (size_t)nF * 12);
+    SCN_ALLOC(keep, (size_t)nF * 4); SCN_ALLOC(fpos, ((size_t)nF + 1) * 4); SCN_ALLOC(ktri, (size_t)nF * 12);
     k_piece_keep<<<grid_for(nF), 256, 0, st>>>(m.tri.as<unsigned>(), nF, root.as<unsigned>(), vcount.as<unsigned>(), fcount.as<unsigned>(), min_v, min_f,
                                                keep.as<unsigned>());
     scn::exclusive_scan_u32(keep.as<unsigned>(), fpos.as<unsigned>(), nF, s.scr.as<unsigned>(), st);
@@ -434,17 +447,17 @@ int step_pieces(Mesh& m, unsigned min_v, unsigned min_f, Scratch& s, scn_mesh_cl
   rep.pieces_total = h_small[0]; rep.pieces_removed = h_small[1]; rep.faces_in_removed_pieces = h_small[2];
   // removeIsolatedVertices: vertices numbered by their first corner in the surviving faces
   const unsigned nC = 3 * nF2;
-  MC_ALLOC(otri, (size_t)nC * 4);
+  SCN_ALLOC(otri, (size_t)nC * 4);
   if (nC) {
-    MC_ALLOC(first, (size_t)n * 4); MC_ALLOC(flag, (size_t)nC * 4); MC_ALLOC(cpos, ((size_t)nC + 1) * 4);
+    SCN_ALLOC(first, (size_t)n * 4); SCN_ALLOC(flag, (size_t)nC * 4); SCN_ALLOC(cpos, ((size_t)nC + 1) * 4);
     SCN_CUDA_TRY(cudaMemsetAsync(first.p, 0xFF, (size_t)n * 4, st));
     k_first_corner<<<grid_for(nC), 256, 0, st>>>(ktri.as<unsigned>(), nC, first.as<unsigned>());
     k_first_flags<<<grid_for(nC), 256, 0, st>>>(ktri.as<unsigned>(), nC, first.as<unsigned>(), flag.as<unsigned>());
     scn::exclusive_scan_u32(flag.as<unsigned>(), cpos.as<unsigned>(), nC, s.scr.as<unsigned>(), st);
     if (int rc = read_u32(cpos.as<unsigned>() + nC, &nV2, 1, st)) return rc;
   }
-  MC_ALLOC(oxyz, (size_t)nV2 * 12);
-  if (m.has_rgb) MC_ALLOC(orgb, (size_t)nV2 * 3);
+  SCN_ALLOC(oxyz, (size_t)nV2 * 12);
+  if (m.has_rgb) SCN_ALLOC(orgb, (size_t)nV2 * 3);
   if (nC)
     k_renumber<<<grid_for(nC), 256, 0, st>>>(ktri.as<unsigned>(), nC, first.as<unsigned>(), flag.as<unsigned>(), cpos.as<unsigned>(), m.xyz.as<float>(),
                                             m.rgb.as<unsigned char>(), otri.as<unsigned>(), oxyz.as<float>(), orgb.as<unsigned char>());
@@ -458,8 +471,8 @@ int drop_unreferenced(Mesh& m, Scratch& s, cudaStream_t st, unsigned* h_small) {
   const unsigned n = m.nV, nC = 3 * m.nF;
   if (int rc = s.ensure(1, (size_t)n + 1)) return rc;
   DBuf used, newid, ident, keep, otri, oxyz, orgb;
-  MC_ALLOC(used, (size_t)n * 4); MC_ALLOC(newid, ((size_t)n + 1) * 4); MC_ALLOC(ident, (size_t)n * 4); MC_ALLOC(keep, (size_t)m.nF * 4);
-  MC_ALLOC(otri, (size_t)nC * 4);
+  SCN_ALLOC(used, (size_t)n * 4); SCN_ALLOC(newid, ((size_t)n + 1) * 4); SCN_ALLOC(ident, (size_t)n * 4); SCN_ALLOC(keep, (size_t)m.nF * 4);
+  SCN_ALLOC(otri, (size_t)nC * 4);
   unsigned nV2 = 0;
   if (n) {
     SCN_CUDA_TRY(cudaMemsetAsync(used.p, 0, (size_t)n * 4, st));
@@ -469,8 +482,8 @@ int drop_unreferenced(Mesh& m, Scratch& s, cudaStream_t st, unsigned* h_small) {
     if (int rc = read_u32(newid.as<unsigned>() + n, h_small, 1, st)) return rc;
     nV2 = h_small[0];
   }
-  MC_ALLOC(oxyz, (size_t)nV2 * 12);
-  if (m.has_rgb) MC_ALLOC(orgb, (size_t)nV2 * 3);
+  SCN_ALLOC(oxyz, (size_t)nV2 * 12);
+  if (m.has_rgb) SCN_ALLOC(orgb, (size_t)nV2 * 3);
   if (n) k_merge_vertices<<<grid_for(n), 256, 0, st>>>(m.xyz.as<float>(), m.rgb.as<unsigned char>(), used.as<unsigned>(), newid.as<unsigned>(), n,
                                                        oxyz.as<float>(), orgb.as<unsigned char>());
   if (m.nF) k_merge_faces<<<grid_for(m.nF), 256, 0, st>>>(m.tri.as<unsigned>(), m.nF, ident.as<unsigned>(), newid.as<unsigned>(), otri.as<unsigned>(),
@@ -482,24 +495,25 @@ int drop_unreferenced(Mesh& m, Scratch& s, cudaStream_t st, unsigned* h_small) {
 }
 
 int run_clean_steps(Mesh& m, const scn_mesh_clean_params& params, Scratch& s, scn_mesh_clean_report_t& rep, cudaStream_t st,
-                    unsigned* d_err, unsigned* h_small, const cudaEvent_t* ev) {
+                    unsigned* d_err, unsigned* h_small, const EventPtr* ev) {
   int rc = SCN_OK;
   if (!(params.flags & SCN_CLEAN_SKIP_MERGE)) rc = step_merge(m, params.merge_threshold, s, rep, st, d_err, h_small);
   if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(ev[1], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[1].get(), st));
   if (!(params.flags & SCN_CLEAN_SKIP_DEDUP)) rc = step_dedup(m, s, rep, st);
   if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(ev[2], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[2].get(), st));
   if (!(params.flags & SCN_CLEAN_SKIP_PIECES)) rc = step_pieces(m, params.min_piece_vertices, params.min_piece_faces, s, rep, st, h_small);
   if (rc) return rc;
-  SCN_CUDA_TRY(cudaEventRecord(ev[3], st));
-  SCN_CUDA_TRY(cudaEventSynchronize(ev[3]));
+  SCN_CUDA_TRY(cudaEventRecord(ev[3].get(), st));
+  SCN_CUDA_TRY(cudaEventSynchronize(ev[3].get()));
   rep.merge_ms = ms_between(ev[0], ev[1]); rep.dedup_ms = ms_between(ev[1], ev[2]); rep.pieces_ms = ms_between(ev[2], ev[3]);
   return SCN_OK;
 }
 
 }  // namespace scn::mc
 
+using namespace scn;
 using namespace scn::mc;
 
 extern "C" {
@@ -528,41 +542,21 @@ int scn_mesh_clean(const float* xyz, const uint8_t* rgb, uint64_t nV, const uint
   memset(&rep, 0, sizeof(rep));
   rep.vertices_in = nV; rep.faces_in = nF;
   const auto t0 = std::chrono::steady_clock::now();
-  Stream S;
-  SCN_CUDA_TRY(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
-  for (auto& e : S.ev) SCN_CUDA_TRY(cudaEventCreate(&e));
-  const cudaStream_t st = S.s;
-  Mesh m; Scratch s; DBuf err;
-  unsigned* h_small = nullptr;
-  SCN_CUDA_TRY(cudaMallocHost(&h_small, 16));
-  struct HostFree { unsigned* p; ~HostFree() { cudaFreeHost(p); } } hf{h_small};
-  m.nV = (unsigned)nV; m.nF = (unsigned)nF; m.has_rgb = rgb != nullptr;
-  MC_ALLOC(m.xyz, nV * 12); MC_ALLOC(m.tri, nF * 12); MC_ALLOC(err, 4);
-  if (m.has_rgb) MC_ALLOC(m.rgb, nV * 3);
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[0], st));
-  if (nV) SCN_CUDA_TRY(cudaMemcpyAsync(m.xyz.p, xyz, nV * 12, cudaMemcpyHostToDevice, st));
-  if (nV && rgb) SCN_CUDA_TRY(cudaMemcpyAsync(m.rgb.p, rgb, nV * 3, cudaMemcpyHostToDevice, st));
-  if (nF) SCN_CUDA_TRY(cudaMemcpyAsync(m.tri.p, tri, nF * 12, cudaMemcpyHostToDevice, st));
-  SCN_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, st));
+  StreamPtr S; EventPtr ev[6];
+  SCN_CUDA_TRY(create(S, ev, 6));
+  const cudaStream_t st = S.get();
+  Mesh m; Scratch s; DBuf err; PinnedPtr<unsigned> h_small;
+  if (int rc = upload_mesh(m, xyz, rgb, nV, tri, nF, h_small, err, ev[0].get(), st)) return rc;
   if (nF) k_check_faces<<<grid_for(3 * nF), 256, 0, st>>>(m.tri.as<unsigned>(), 3 * nF, (unsigned)nV, err.as<unsigned>());
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[1], st));
-  if (int rc = read_u32(err.as<unsigned>(), h_small, 1, st)) return rc;
+  SCN_CUDA_TRY(cudaEventRecord(ev[1].get(), st));
+  if (int rc = read_u32(err.as<unsigned>(), h_small.get(), 1, st)) return rc;
   if (h_small[0] & ERR_INDEX) return scn::fail(SCN_ERR_ARG, "scn_mesh_clean: a face references a vertex >= %llu", (unsigned long long)nV);
-  if (int rc = run_clean_steps(m, *params, s, rep, st, err.as<unsigned>(), h_small, S.ev + 1)) return rc;
-  float* hx = (float*)malloc(std::max<size_t>((size_t)m.nV * 12, 1));
-  uint32_t* ht = (uint32_t*)malloc(std::max<size_t>((size_t)m.nF * 12, 1));
-  uint8_t* hc = rgb && rgb_out ? (uint8_t*)malloc(std::max<size_t>((size_t)m.nV * 3, 1)) : nullptr;
-  auto bail = [&](int code) { free(hx); free(ht); free(hc); return code; };
-  if (!hx || !ht || (rgb && rgb_out && !hc)) return bail(scn::fail(SCN_ERR_ARG, "scn_mesh_clean: out of host memory"));
-  if ((m.nV && cudaMemcpyAsync(hx, m.xyz.p, (size_t)m.nV * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      (m.nF && cudaMemcpyAsync(ht, m.tri.p, (size_t)m.nF * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      (hc && m.nV && cudaMemcpyAsync(hc, m.rgb.p, (size_t)m.nV * 3, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      cudaEventRecord(S.ev[5], st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
-    return bail(scn::fail(SCN_ERR_CUDA, "scn_mesh_clean: download failed: %s", cudaGetErrorString(cudaGetLastError())));
+  if (int rc = run_clean_steps(m, *params, s, rep, st, err.as<unsigned>(), h_small.get(), ev + 1)) return rc;
+  if (int rc = download_mesh(m, xyz_out, rgb_out, tri_out, ev[5].get(), st, "scn_mesh_clean")) return rc;
   rep.vertices_out = m.nV; rep.faces_out = m.nF;
-  rep.upload_ms = ms_between(S.ev[0], S.ev[1]); rep.download_ms = ms_between(S.ev[4], S.ev[5]);
+  rep.upload_ms = ms_between(ev[0], ev[1]); rep.download_ms = ms_between(ev[4], ev[5]);
   rep.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  *xyz_out = hx; *tri_out = ht; if (rgb_out) *rgb_out = hc; *nV_out = m.nV; *nF_out = m.nF;
+  *nV_out = m.nV; *nF_out = m.nF;
   if (report) *report = rep;
   return SCN_OK;
 }

@@ -30,9 +30,8 @@
 
 namespace {
 
+using namespace scn;
 using namespace scn::mc;
-using scn::bits_for;
-using scn::k_iota;
 
 __device__ __forceinline__ size_t tid() { return blockIdx.x * (size_t)blockDim.x + threadIdx.x; }
 
@@ -380,51 +379,38 @@ int scn_mesh_simplify(const float* xyz, const uint8_t* rgb, uint64_t nV, const u
   memset(&rep, 0, sizeof(rep));
   rep.vertices_in = nV; rep.faces_in = nF; rep.target_faces = target;
   const auto t0 = std::chrono::steady_clock::now();
-  Stream S;
-  SCN_CUDA_TRY(cudaStreamCreateWithFlags(&S.s, cudaStreamNonBlocking));
-  for (auto& e : S.ev) SCN_CUDA_TRY(cudaEventCreate(&e));
-  cudaEvent_t cev[4] = {};
-  struct EvFree { cudaEvent_t* e; ~EvFree() { for (int i = 0; i < 4; ++i) if (e[i]) cudaEventDestroy(e[i]); } } ef{cev};
-  for (auto& e : cev) SCN_CUDA_TRY(cudaEventCreate(&e));
-  const cudaStream_t st = S.s;
-  Mesh m; Scratch s; Work w; DBuf err;
-  unsigned* h_small = nullptr;
-  SCN_CUDA_TRY(cudaMallocHost(&h_small, 16));
-  struct HostFree { unsigned* p; ~HostFree() { cudaFreeHost(p); } } hf{h_small};
-  m.nV = (unsigned)nV; m.nF = (unsigned)nF; m.has_rgb = rgb != nullptr;
+  StreamPtr S; EventPtr ev[11];                 // ev[7..10]: the clean filters' steps
+  SCN_CUDA_TRY(create(S, ev, 11));
+  const cudaStream_t st = S.get();
+  Mesh m; Scratch s; Work w; DBuf err; PinnedPtr<unsigned> hp;
   const size_t nC = 3 * (size_t)nF;
-  MC_ALLOC(m.xyz, nV * 12); MC_ALLOC(m.tri, nF * 12); MC_ALLOC(err, 4);
-  if (m.has_rgb) MC_ALLOC(m.rgb, nV * 3);
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[0], st));
-  if (nV) SCN_CUDA_TRY(cudaMemcpyAsync(m.xyz.p, xyz, nV * 12, cudaMemcpyHostToDevice, st));
-  if (nV && rgb) SCN_CUDA_TRY(cudaMemcpyAsync(m.rgb.p, rgb, nV * 3, cudaMemcpyHostToDevice, st));
-  if (nF) SCN_CUDA_TRY(cudaMemcpyAsync(m.tri.p, tri, nF * 12, cudaMemcpyHostToDevice, st));
-  SCN_CUDA_TRY(cudaMemsetAsync(err.p, 0, 4, st));
+  if (int rc = upload_mesh(m, xyz, rgb, nV, tri, nF, hp, err, ev[0].get(), st)) return rc;
+  unsigned* h_small = hp.get();
   if (nV || nF) k_check<<<grid_for(std::max<size_t>(3 * nV, nC)), 256, 0, st>>>(m.xyz.as<float>(), 3 * nV, m.tri.as<unsigned>(), nC, (unsigned)nV,
                                                                                 err.as<unsigned>());
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[1], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[1].get(), st));
   if (int rc = read_u32(err.as<unsigned>(), h_small, 1, st)) return rc;
   if (h_small[0] & ERR_INDEX) return scn::fail(SCN_ERR_ARG, "scn_mesh_simplify: a face references a vertex >= %llu", (unsigned long long)nV);
   if (h_small[0] & ERR_COORD) return scn::fail(SCN_ERR_ARG, "scn_mesh_simplify: a vertex coordinate is not finite");
   // per-round buffers, sized for the input (every round has at most nC corners and edges)
   if (int rc = s.ensure(std::max<size_t>(nC, 1), nC + 1)) return rc;
-  MC_ALLOC(w.Q, nV * 80); MC_ALLOC(w.rs, nV * 4); MC_ALLOC(w.re, nV * 4); MC_ALLOC(w.ring, nC * 4); MC_ALLOC(w.head, nC * 4);
-  MC_ALLOC(w.hidx, (nC + 1) * 4); MC_ALLOC(w.ea, nC * 4); MC_ALLOC(w.eb, nC * 4); MC_ALLOC(w.cost, nC * 8); MC_ALLOC(w.pstar, nC * 12);
-  MC_ALLOC(w.fcount, nC * 4); MC_ALLOC(w.rank, nC * 4); MC_ALLOC(w.m, nV * 4); MC_ALLOC(w.M, nV * 4); MC_ALLOC(w.sf, nC * 4);
-  MC_ALLOC(w.pre, (nC + 1) * 4); MC_ALLOC(w.remap, nV * 4); MC_ALLOC(w.keep, nF * 4); MC_ALLOC(w.fpos, (nF + 1) * 4); MC_ALLOC(w.otri, nF * 12);
-  MC_ALLOC(w.big, 4); MC_ALLOC(w.counters, 16);
+  SCN_ALLOC(w.Q, nV * 80); SCN_ALLOC(w.rs, nV * 4); SCN_ALLOC(w.re, nV * 4); SCN_ALLOC(w.ring, nC * 4); SCN_ALLOC(w.head, nC * 4);
+  SCN_ALLOC(w.hidx, (nC + 1) * 4); SCN_ALLOC(w.ea, nC * 4); SCN_ALLOC(w.eb, nC * 4); SCN_ALLOC(w.cost, nC * 8); SCN_ALLOC(w.pstar, nC * 12);
+  SCN_ALLOC(w.fcount, nC * 4); SCN_ALLOC(w.rank, nC * 4); SCN_ALLOC(w.m, nV * 4); SCN_ALLOC(w.M, nV * 4); SCN_ALLOC(w.sf, nC * 4);
+  SCN_ALLOC(w.pre, (nC + 1) * 4); SCN_ALLOC(w.remap, nV * 4); SCN_ALLOC(w.keep, nF * 4); SCN_ALLOC(w.fpos, (nF + 1) * 4); SCN_ALLOC(w.otri, nF * 12);
+  SCN_ALLOC(w.big, 4); SCN_ALLOC(w.counters, 16);
   SCN_CUDA_TRY(cudaMemsetAsync(w.big.p, 0, 4, st)); SCN_CUDA_TRY(cudaMemsetAsync(w.counters.p, 0, 16, st));
   if (int rc = build_ring(m, s, w, st, false)) return rc;
   if (nV) k_vertex_quadrics<<<grid_for(nV), 256, 0, st>>>(w.rs.as<unsigned>(), w.re.as<unsigned>(), w.ring.as<unsigned>(), m.tri.as<unsigned>(),
                                                           m.xyz.as<float>(), (unsigned)nV, w.Q.as<double>());
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[2], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[2].get(), st));
   while (m.nF > target) {
     bool applied = false;
     if (int rc = run_round(m, s, w, params->quality_thr, target, st, h_small, &applied)) return rc;
     if (!applied) break;
     ++rep.rounds;
   }
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[3], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[3].get(), st));
   {
     unsigned long long c[2];
     SCN_CUDA_TRY(cudaMemcpyAsync(c, w.counters.p, 16, cudaMemcpyDeviceToHost, st));
@@ -443,29 +429,20 @@ int scn_mesh_simplify(const float* xyz, const uint8_t* rgb, uint64_t nV, const u
     rep.autoclean_duplicate_faces = dup.duplicate_faces;
     if (int rc = drop_unreferenced(m, s, st, h_small)) return rc;
   }
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[4], st));
-  SCN_CUDA_TRY(cudaEventRecord(cev[0], st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[4].get(), st));
+  SCN_CUDA_TRY(cudaEventRecord(ev[7].get(), st));
   if (after) {
     rep.clean.vertices_in = m.nV; rep.clean.faces_in = m.nF;
-    if (int rc = run_clean_steps(m, *after, s, rep.clean, st, err.as<unsigned>(), h_small, cev)) return rc;
+    if (int rc = run_clean_steps(m, *after, s, rep.clean, st, err.as<unsigned>(), h_small, ev + 7)) return rc;
     rep.clean.vertices_out = m.nV; rep.clean.faces_out = m.nF;
   }
-  SCN_CUDA_TRY(cudaEventRecord(S.ev[5], st));
-  float* hx = (float*)malloc(std::max<size_t>((size_t)m.nV * 12, 1));
-  uint32_t* ht = (uint32_t*)malloc(std::max<size_t>((size_t)m.nF * 12, 1));
-  uint8_t* hc = rgb && rgb_out ? (uint8_t*)malloc(std::max<size_t>((size_t)m.nV * 3, 1)) : nullptr;
-  auto bail = [&](int code) { free(hx); free(ht); free(hc); return code; };
-  if (!hx || !ht || (rgb && rgb_out && !hc)) return bail(scn::fail(SCN_ERR_ARG, "scn_mesh_simplify: out of host memory"));
-  if ((m.nV && cudaMemcpyAsync(hx, m.xyz.p, (size_t)m.nV * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      (m.nF && cudaMemcpyAsync(ht, m.tri.p, (size_t)m.nF * 12, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      (hc && m.nV && cudaMemcpyAsync(hc, m.rgb.p, (size_t)m.nV * 3, cudaMemcpyDeviceToHost, st) != cudaSuccess) ||
-      cudaEventRecord(S.ev[6], st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
-    return bail(scn::fail(SCN_ERR_CUDA, "scn_mesh_simplify: download failed: %s", cudaGetErrorString(cudaGetLastError())));
+  SCN_CUDA_TRY(cudaEventRecord(ev[5].get(), st));
+  if (int rc = download_mesh(m, xyz_out, rgb_out, tri_out, ev[6].get(), st, "scn_mesh_simplify")) return rc;
   rep.vertices_out = m.nV; rep.faces_out = m.nF;
-  rep.upload_ms = ms_between(S.ev[0], S.ev[1]); rep.quadrics_ms = ms_between(S.ev[1], S.ev[2]); rep.rounds_ms = ms_between(S.ev[2], S.ev[3]);
-  rep.autoclean_ms = ms_between(S.ev[3], S.ev[4]); rep.clean_ms = ms_between(S.ev[4], S.ev[5]); rep.download_ms = ms_between(S.ev[5], S.ev[6]);
+  rep.upload_ms = ms_between(ev[0], ev[1]); rep.quadrics_ms = ms_between(ev[1], ev[2]); rep.rounds_ms = ms_between(ev[2], ev[3]);
+  rep.autoclean_ms = ms_between(ev[3], ev[4]); rep.clean_ms = ms_between(ev[4], ev[5]); rep.download_ms = ms_between(ev[5], ev[6]);
   rep.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  *xyz_out = hx; *tri_out = ht; if (rgb_out) *rgb_out = hc; *nV_out = m.nV; *nF_out = m.nF;
+  *nV_out = m.nV; *nF_out = m.nF;
   if (report) *report = rep;
   return SCN_OK;
 }

@@ -1,9 +1,13 @@
 // Stable LSD radix sort of (uint32 key, uint32 value) pairs (hand-written: per-tile digit histograms, one device-wide scan,
-// rank-preserving scatter), 8 bits per pass.  Shared by segs.cu and meshclean.cu.
+// rank-preserving scatter), 8 bits per pass, and the scratch its callers sort in.  Shared by segs.cu, meshclean.cu and
+// meshsimplify.cu.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
+
 #include "scan.cuh"
+#include "scn_common.h"
 
 namespace scn {
 
@@ -76,5 +80,30 @@ inline size_t rs_hist_elems(size_t n) { return (size_t)256 * ((n + kRsTile - 1) 
 inline int bits_for(unsigned maxv) { int b = 1; while (b < 32 && (maxv >> b)) ++b; return b; }
 
 static __global__ void k_iota(unsigned* v, size_t n) { const size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; if (i < n) v[i] = (unsigned)i; }
+
+struct Scratch {                      // radix-sort pairs and scan scratch, grown on demand
+  DBuf k0, v0, k1, v1, hist, scr;
+  size_t cap_pairs = 0, cap_scan = 0;
+  int ensure(size_t n, size_t scan_n) {          // sorts of n pairs, scans of up to scan_n elements
+    if (n > cap_pairs) {
+      SCN_ALLOC(k0, n * 4); SCN_ALLOC(v0, n * 4); SCN_ALLOC(k1, n * 4); SCN_ALLOC(v1, n * 4); SCN_ALLOC(hist, rs_hist_elems(n) * 4);
+      cap_pairs = n;
+    }
+    const size_t need = scan_scratch_elems(std::max(rs_hist_elems(cap_pairs), scan_n));
+    if (need > cap_scan) { SCN_ALLOC(scr, need * 4); cap_scan = need; }
+    return SCN_OK;
+  }
+};
+
+// sorts `vals` (initially any permutation) stably by the keys staged in s.k0, leaving the result in (k0,v0) or (k1,v1);
+// returns the value array
+inline unsigned* sort_pass(Scratch& s, unsigned*& vals, size_t n, int bits, cudaStream_t st) {
+  unsigned* k0 = s.k0.as<unsigned>(); unsigned* k1 = s.k1.as<unsigned>();
+  unsigned* v0 = s.v0.as<unsigned>(); unsigned* v1 = s.v1.as<unsigned>();
+  if (vals != v0) { cudaMemcpyAsync(v0, vals, n * 4, cudaMemcpyDeviceToDevice, st); }
+  const int w = radix_sort_pairs(k0, v0, k1, v1, n, bits, s.hist.as<unsigned>(), s.scr.as<unsigned>(), st);
+  vals = w ? v1 : v0;
+  return vals;
+}
 
 }  // namespace scn

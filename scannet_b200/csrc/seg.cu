@@ -573,9 +573,6 @@ __global__ void k_compact_edges(const Rec* __restrict__ rec, const unsigned* __r
 }
 
 // ------------------------------------------------------------------------------ host side
-#define CK(expr) do { cudaError_t _e = (expr); if (_e != cudaSuccess) { \
-  scn::fail(SCN_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); return SCN_ERR_CUDA; } } while (0)
-
 // Workspace: a per-thread cached device arena (bump allocator).  cudaMalloc/cudaFree cost ~0.1-1 ms each and
 // synchronise the device; with ~25 buffers per call they dominated small meshes.  The arena is reset at the start of
 // every top-level call and regrown to a single chunk when a call overflowed it.
@@ -639,21 +636,21 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
   unsigned* smStart = bSm.as<unsigned>(); unsigned* smLenD = smStart + maxSmall;
   unsigned* hpStart = bHp.as<unsigned>(); unsigned* hpEnd = hpStart + maxLarge;
   SortCtl* ctl = bCtl.as<SortCtl>();
-  CK(cudaMemsetAsync(ctl, 0, sizeof(SortCtl), st));
+  SCN_CUDA_TRY(cudaMemsetAsync(ctl, 0, sizeof(SortCtl), st));
   SortCtl h{};
   unsigned nseg = 0;
   int cur = 0;
   if (n <= (size_t)kSmall) {
     const unsigned s0 = 0, ld = ((unsigned)n << 8) | depth0;
-    CK(cudaMemcpyAsync(smStart, &s0, 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(smLenD, &ld, 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(smStart, &s0, 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(smLenD, &ld, 4, cudaMemcpyHostToDevice, st));
     h.n_small = 1;
   } else {
     const unsigned init[3] = { 0u, (unsigned)n, depth0 };
     unsigned* S = bSeg[0].as<unsigned>();
-    CK(cudaMemcpyAsync(S, &init[0], 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(S + maxLarge, &init[1], 4, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(S + 2 * maxLarge, &init[2], 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(S, &init[0], 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(S + maxLarge, &init[1], 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(S + 2 * maxLarge, &init[2], 4, cudaMemcpyHostToDevice, st));
     nseg = 1;
   }
   static const bool by_launches = getenv("SCN_SEG_SORT_LAUNCHES") != nullptr;      // the per-level launch sequence, kept for A/B timing
@@ -664,10 +661,10 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
     static thread_local int coop_blocks = 0;
     if (!coop_blocks) {
       int dev = 0, sms = 0, occ = 0, coop = 0;
-      CK(cudaGetDevice(&dev));
-      CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-      CK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_sort_levels, kTileThreads, 0));
+      SCN_CUDA_TRY(cudaGetDevice(&dev));
+      SCN_CUDA_TRY(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+      SCN_CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+      SCN_CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_sort_levels, kTileThreads, 0));
       coop_blocks = coop ? sms * std::max(1, std::min(occ, 2)) : -1;
     }
     if (coop_blocks > 0) {
@@ -675,7 +672,7 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
       const int use_blocks = (int)std::max<size_t>(1, std::min<size_t>((size_t)coop_blocks, (n + kTile - 1) / kTile));
       DevBuf bBar;
       if (bBar.alloc(16)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc (sort barrier)");
-      CK(cudaMemsetAsync(bBar.p, 0, 16, st));
+      SCN_CUDA_TRY(cudaMemsetAsync(bBar.p, 0, 16, st));
       SortLevelsArgs a;
       a.A = A; a.seg[0] = bSeg[0].as<unsigned>(); a.seg[1] = bSeg[1].as<unsigned>(); a.maxLarge = (unsigned)maxLarge;
       a.cut = bCut.as<unsigned>(); a.tileCnt = bTileCnt.as<unsigned>(); a.tileOff = bTileOff.as<unsigned>();
@@ -683,10 +680,10 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
       a.Lpos = bLpos.as<unsigned>(); a.Rpos = bRpos.as<unsigned>(); a.smStart = smStart; a.smLenD = smLenD; a.hpStart = hpStart; a.hpEnd = hpEnd;
       a.ctl = ctl; a.bar = bBar.as<unsigned>(); a.nseg0 = nseg;
       void* params[] = { (void*)&a };
-      CK(cudaLaunchCooperativeKernel((const void*)k_sort_levels, dim3((unsigned)use_blocks), dim3(kTileThreads), params, 0, st));
+      SCN_CUDA_TRY(cudaLaunchCooperativeKernel((const void*)k_sort_levels, dim3((unsigned)use_blocks), dim3(kTileThreads), params, 0, st));
       g_sort_launches += 1;
-      CK(cudaMemcpyAsync(&h, ctl, sizeof(SortCtl), cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
+      SCN_CUDA_TRY(cudaMemcpyAsync(&h, ctl, sizeof(SortCtl), cudaMemcpyDeviceToHost, st));
+      SCN_CUDA_TRY(cudaStreamSynchronize(st));
       nseg = 0;
     }
   }
@@ -697,8 +694,8 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
     k_pivot<<<gb, 128, 0, st>>>(A, S, E, nseg, bTileCnt.as<unsigned>());
     g_sort_launches += 1 + scn::exclusive_scan_u32(bTileCnt.as<unsigned>(), bTileOff.as<unsigned>(), nseg, bScr.as<unsigned>(), st);
     unsigned ntiles = 0;
-    CK(cudaMemcpyAsync(&ntiles, bTileOff.as<unsigned>() + nseg, 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(&ntiles, bTileOff.as<unsigned>() + nseg, 4, cudaMemcpyDeviceToHost, st));
+    SCN_CUDA_TRY(cudaStreamSynchronize(st));
     k_count<<<ntiles, kTileThreads, 0, st>>>(A, S, E, bTileOff.as<unsigned>(), nseg, bTL.as<unsigned>(), bTR.as<unsigned>());
     g_sort_launches += 1 + scn::exclusive_scan_u32(bTL.as<unsigned>(), bGL.as<unsigned>(), ntiles, bScr.as<unsigned>(), st);
     g_sort_launches += scn::exclusive_scan_u32(bTR.as<unsigned>(), bGR.as<unsigned>(), ntiles, bScr.as<unsigned>(), st);
@@ -708,16 +705,16 @@ int device_introsort(Rec* A, size_t n, cudaStream_t st, int forced_depth = 0) {
                                               bLpos.as<unsigned>(), bRpos.as<unsigned>(), bCut.as<unsigned>());
     k_children<<<gb, 128, 0, st>>>(S, E, D, bCut.as<unsigned>(), nseg, NS, NE, ND, smStart, smLenD, hpStart, hpEnd, ctl);
     g_sort_launches += 3;
-    CK(cudaMemcpyAsync(&h, ctl, sizeof(SortCtl), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(&h, ctl, sizeof(SortCtl), cudaMemcpyDeviceToHost, st));
+    SCN_CUDA_TRY(cudaStreamSynchronize(st));
     nseg = h.n_next;
     const unsigned zero = 0;
-    CK(cudaMemcpyAsync(&ctl->n_next, &zero, 4, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(&ctl->n_next, &zero, 4, cudaMemcpyHostToDevice, st));
     cur ^= 1;
   }
   if (h.n_heap) { k_sort_heap_fallback<<<(h.n_heap + 63) / 64, 64, 0, st>>>(A, hpStart, hpEnd, h.n_heap); ++g_sort_launches; }
   if (h.n_small) { k_sort_small<<<(h.n_small + kSmallWarps - 1) / kSmallWarps, 32 * kSmallWarps, 0, st>>>(A, smStart, smLenD, h.n_small); ++g_sort_launches; }
-  CK(cudaGetLastError());
+  SCN_CUDA_TRY(cudaGetLastError());
   return SCN_OK;
 }
 
@@ -882,10 +879,10 @@ int device_kruskal(const Edge12* dE, size_t nK, size_t nV, float c, Forest& u, c
   if (dU.alloc(nV * sizeof(UfElt)) || dOwner.alloc(nV * 4) || dRounds.alloc(8)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc (device union-find)");
   k_uf_init<<<(unsigned)((nV + 255) / 256), 256, 0, st>>>(dU.as<UfElt>(), dOwner.as<int>(), nV, c);
   k_kruskal_window<<<1, kUfWindow, 0, st>>>(dE, (unsigned)nK, dU.as<UfElt>(), dOwner.as<int>(), c, dRounds.as<unsigned long long>());
-  CK(cudaMemcpyAsync(u.data(), dU.p, nV * sizeof(UfElt), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(&g_uf_rounds, dRounds.p, 8, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  CK(cudaGetLastError());
+  SCN_CUDA_TRY(cudaMemcpyAsync(u.data(), dU.p, nV * sizeof(UfElt), cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(&g_uf_rounds, dRounds.p, 8, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaGetLastError());
   return SCN_OK;
 }
 
@@ -899,21 +896,21 @@ int prune_and_download(const Rec* dRec, const unsigned* dTri, const Edge12* dSrc
   DevBuf dK, dM, dKeep, dPos, dOut, dScr;
   if (dK.alloc(cap * 8) || dM.alloc(cap * 4) || dKeep.alloc(nE * 4) || dPos.alloc((nE + 1) * 4) || dOut.alloc(nE * 12) || dScr.alloc(scn::scan_scratch_elems(nE) * 4))
     return scn::fail(SCN_ERR_CUDA, "cudaMalloc (replay pruning workspace)");
-  CK(cudaMemsetAsync(dK.p, 0xFF, cap * 8, st));
-  CK(cudaMemsetAsync(dM.p, 0xFF, cap * 4, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(dK.p, 0xFF, cap * 8, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(dM.p, 0xFF, cap * 4, st));
   const unsigned g = (unsigned)((nE + 255) / 256);
   k_pair_first<<<g, 256, 0, st>>>(dRec, dTri, dSrc, nE, dK.as<unsigned long long>(), dM.as<unsigned>(), (unsigned)(cap - 1));
   k_pair_keep<<<g, 256, 0, st>>>(dRec, dTri, dSrc, nE, dK.as<unsigned long long>(), dM.as<unsigned>(), (unsigned)(cap - 1), dKeep.as<unsigned>());
   scn::exclusive_scan_u32(dKeep.as<unsigned>(), dPos.as<unsigned>(), nE, dScr.as<unsigned>(), st);
   k_compact_edges<<<g, 256, 0, st>>>(dRec, dTri, dSrc, nE, dKeep.as<unsigned>(), dPos.as<unsigned>(), dOut.as<Edge12>());
   unsigned nk = 0;
-  CK(cudaMemcpyAsync(&nk, dPos.as<unsigned>() + nE, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(&nk, dPos.as<unsigned>() + nE, 4, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   void* h = g_pinned.get((size_t)nk * 12 + 16);
   if (!h) return scn::fail(SCN_ERR_CUDA, "cudaHostAlloc (%u records)", nk);
-  CK(cudaMemcpyAsync(h, dOut.p, (size_t)nk * 12, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  CK(cudaGetLastError());
+  SCN_CUDA_TRY(cudaMemcpyAsync(h, dOut.p, (size_t)nk * 12, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaGetLastError());
   *out = (const Edge12*)h; *n_out = nk; if (d_out) *d_out = dOut.as<Edge12>();
   return SCN_OK;
 }
@@ -950,20 +947,20 @@ int filter_small_merge(const Edge12* dE, size_t nK, const Forest& u, int min_ver
   DevBuf dPs, dRoot, dKeep, dPos, dOut, dScr;
   if (dPs.alloc(nV * 8) || dRoot.alloc(nV * 4) || dKeep.alloc(nK * 4) || dPos.alloc((nK + 1) * 4) || dOut.alloc(nK * 12) || dScr.alloc(scn::scan_scratch_elems(nK) * 4))
     return scn::fail(SCN_ERR_CUDA, "cudaMalloc (small-segment filter workspace)");
-  CK(cudaMemcpyAsync(dPs.p, hps, nV * 8, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dPs.p, hps, nV * 8, cudaMemcpyHostToDevice, st));
   k_uf_roots<<<(unsigned)((nV + 255) / 256), 256, 0, st>>>(dPs.as<int2>(), nV, dRoot.as<int>());
   const unsigned g = (unsigned)((nK + 255) / 256);
   k_small_keep<<<g, 256, 0, st>>>(dE, nK, dRoot.as<int>(), dPs.as<int2>(), min_verts, dKeep.as<unsigned>());
   scn::exclusive_scan_u32(dKeep.as<unsigned>(), dPos.as<unsigned>(), nK, dScr.as<unsigned>(), st);
   k_compact12<<<g, 256, 0, st>>>(dE, nK, dKeep.as<unsigned>(), dPos.as<unsigned>(), dOut.as<Edge12>());
   unsigned n2 = 0;
-  CK(cudaMemcpyAsync(&n2, dPos.as<unsigned>() + nK, 4, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(&n2, dPos.as<unsigned>() + nK, 4, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   void* h = g_pinned.get((size_t)n2 * 12 + 16);                 // the Kruskal pass is done with the previous contents
   if (!h) return scn::fail(SCN_ERR_CUDA, "cudaHostAlloc (%u records)", n2);
-  CK(cudaMemcpyAsync(h, dOut.p, (size_t)n2 * 12, cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  CK(cudaGetLastError());
+  SCN_CUDA_TRY(cudaMemcpyAsync(h, dOut.p, (size_t)n2 * 12, cudaMemcpyDeviceToHost, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaGetLastError());
   *out = (const Edge12*)h; *n_out = n2;
   return SCN_OK;
 }
@@ -1018,11 +1015,11 @@ int segment_impl(const float* xyz, uint64_t nV, const uint32_t* tri, uint64_t nF
       dCur.alloc((nV + 1) * 4) || dCsr.alloc(nE * 4) || dNrm.alloc(nV * 12) || dRec.alloc(nE * 8) || dE12.alloc(nE * 12) ||
       dScr.alloc(scn::scan_scratch_elems(nV + 1) * 4))
     return scn::fail(SCN_ERR_CUDA, "cudaMalloc (segmentator workspace)");
-  CK(cudaMemcpyAsync(dXyz.p, src_xyz, nV * 12, cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(dTri.p, src_tri, nF * 12, cudaMemcpyHostToDevice, st));
-  CK(cudaMemsetAsync(dDeg.p, 0, (nV + 1) * 4, st));
-  CK(cudaMemsetAsync(dCur.p, 0, (nV + 1) * 4, st));
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dXyz.p, src_xyz, nV * 12, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemcpyAsync(dTri.p, src_tri, nF * 12, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(dDeg.p, 0, (nV + 1) * 4, st));
+  SCN_CUDA_TRY(cudaMemsetAsync(dCur.p, 0, (nV + 1) * 4, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   g_timings[0] = lapt.lap();
   const unsigned B = 256;
   if (nF) {
@@ -1031,24 +1028,24 @@ int segment_impl(const float* xyz, uint64_t nV, const uint32_t* tri, uint64_t nF
   scn::exclusive_scan_u32(dDeg.as<unsigned>(), dOff.as<unsigned>(), nV, dScr.as<unsigned>(), st);
   if (nF) k_fill_csr<<<(unsigned)((nE + B - 1) / B), B, 0, st>>>(dTri.as<unsigned>(), nF, dOff.as<unsigned>(), dCur.as<unsigned>(), dCsr.as<unsigned>());
   if (nV) k_vertex_normals<<<(unsigned)((nV + 127) / 128), 128, 0, st>>>(dOff.as<unsigned>(), dCsr.as<unsigned>(), dFn.as<float4>(), nV, dNrm.as<float>());
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   g_timings[1] = lapt.lap();
   if (nE) k_edge_weights<<<(unsigned)((nE + B - 1) / B), B, 0, st>>>(dXyz.as<float>(), dTri.as<unsigned>(), dNrm.as<float>(), nE, dRec.as<Rec>());
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   g_timings[2] = lapt.lap();
-  if (normals_out && nV) CK(cudaMemcpy(normals_out, dNrm.p, nV * 12, cudaMemcpyDeviceToHost));
+  if (normals_out && nV) SCN_CUDA_TRY(cudaMemcpy(normals_out, dNrm.p, nV * 12, cudaMemcpyDeviceToHost));
   if (edges_presort && nE) {
     k_gather_edges<<<(unsigned)((nE + B - 1) / B), B, 0, st>>>(dRec.as<Rec>(), dTri.as<unsigned>(), nE, dE12.as<Edge12>());
-    CK(cudaMemcpy(edges_presort, dE12.p, nE * 12, cudaMemcpyDeviceToHost));
+    SCN_CUDA_TRY(cudaMemcpy(edges_presort, dE12.p, nE * 12, cudaMemcpyDeviceToHost));
     lapt.lap();
   }
   int rc = device_introsort(dRec.as<Rec>(), nE, st);
   if (rc) return rc;
-  CK(cudaStreamSynchronize(st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
   g_timings[3] = lapt.lap();
   if (edges_sorted && nE) {                            // full sorted array: parity tests only
     k_gather_edges<<<(unsigned)((nE + B - 1) / B), B, 0, st>>>(dRec.as<Rec>(), dTri.as<unsigned>(), nE, dE12.as<Edge12>());
-    CK(cudaMemcpy(edges_sorted, dE12.p, nE * 12, cudaMemcpyDeviceToHost));
+    SCN_CUDA_TRY(cudaMemcpy(edges_sorted, dE12.p, nE * 12, cudaMemcpyDeviceToHost));
     lapt.lap();
   }
   const Edge12* hE = nullptr; const Edge12* dE = nullptr; size_t nK = 0;
@@ -1100,16 +1097,16 @@ int scn_segment_graph(int32_t n_verts, int64_t n_edges, void* edges, float c, in
   if (dSrc.alloc(nE * 12) || dDst.alloc(nE * 12) || dRec.alloc(nE * 8)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc");
   cudaStream_t st = nullptr;
   if (nE) {
-    CK(cudaMemcpyAsync(dSrc.p, he, nE * 12, cudaMemcpyHostToDevice, st));
+    SCN_CUDA_TRY(cudaMemcpyAsync(dSrc.p, he, nE * 12, cudaMemcpyHostToDevice, st));
     k_rec_from_edges12<<<(unsigned)((nE + 255) / 256), 256, 0, st>>>(dSrc.as<Edge12>(), nE, dRec.as<Rec>());
   }
   int rc = device_introsort(dRec.as<Rec>(), nE, st, (flags >> 8) & 0xFF);
   if (rc) return rc;
   if (nE) {
     k_gather_edges12<<<(unsigned)((nE + 255) / 256), 256, 0, st>>>(dRec.as<Rec>(), dSrc.as<Edge12>(), nE, dDst.as<Edge12>());
-    CK(cudaMemcpy(he, dDst.p, nE * 12, cudaMemcpyDeviceToHost));
+    SCN_CUDA_TRY(cudaMemcpy(he, dDst.p, nE * 12, cudaMemcpyDeviceToHost));
   }
-  CK(cudaGetLastError());
+  SCN_CUDA_TRY(cudaGetLastError());
   const Edge12* hK = nullptr; size_t nK = 0;
   rc = prune_and_download(dRec.as<Rec>(), nullptr, dSrc.as<Edge12>(), nE, st, &hK, &nK);
   if (rc) return rc;

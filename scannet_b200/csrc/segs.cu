@@ -21,19 +21,8 @@
 
 namespace {
 
-struct DBuf {                      // cudaMalloc with scope lifetime (not a hot path: one call per mesh)
-  void* p = nullptr;
-  ~DBuf() { if (p) cudaFree(p); }
-  template <typename T> T* as() const { return (T*)p; }
-  bool alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 4) == cudaSuccess; }
-};
-#define SEGS_ALLOC(buf, bytes) do { if (!(buf).alloc(bytes)) { cudaGetLastError(); return scn::fail(SCN_ERR_CUDA, "cudaMalloc(%zu) failed (%s:%d)", (size_t)(bytes), __FILE__, __LINE__); } } while (0)
-
 // stable LSD radix sort: radix_sort.cuh
-using scn::bits_for;
-using scn::k_iota;
-using scn::radix_sort_pairs;
-using scn::rs_hist_elems;
+using namespace scn;
 
 // ------------------------------------------------------------------------------------------ aggregate
 __global__ void k_heads(const unsigned* __restrict__ sk, size_t n, unsigned* __restrict__ head) {
@@ -245,8 +234,6 @@ __global__ void k_propagate(const float* __restrict__ sxyz, const float* __restr
   out[i] = res;
 }
 
-inline unsigned grid_for(size_t n) { return (unsigned)((n + 255) / 256); }
-
 }  // namespace
 
 extern "C" {
@@ -261,53 +248,52 @@ int scn_segs_aggregate(const uint32_t* seg, uint64_t nV, const float* xyz, const
   unsigned maxv = 0; for (uint64_t i = 0; i < nV; ++i) maxv = std::max(maxv, seg[i]);
   cudaStream_t st = 0;
   const size_t nmax = std::max<size_t>(nV, want_area ? nF : 0);
-  DBuf k0, v0, k1, v1, hist, scr, head, idx, dense, dsegids, doff;
-  SEGS_ALLOC(k0, nmax * 4); SEGS_ALLOC(v0, nmax * 4); SEGS_ALLOC(k1, nmax * 4); SEGS_ALLOC(v1, nmax * 4);
-  SEGS_ALLOC(hist, rs_hist_elems(nmax) * 4); SEGS_ALLOC(scr, scn::scan_scratch_elems(std::max(rs_hist_elems(nmax), nmax + 1)) * 4);
-  SEGS_ALLOC(head, nV * 4); SEGS_ALLOC(idx, (nV + 1) * 4); SEGS_ALLOC(dense, nV * 4); SEGS_ALLOC(dsegids, nV * 4); SEGS_ALLOC(doff, (nV + 1) * 8);
-  SCN_CUDA_TRY(cudaMemcpyAsync(k0.p, seg, nV * 4, cudaMemcpyHostToDevice, st));
-  k_iota<<<grid_for(nV), 256, 0, st>>>(v0.as<unsigned>(), nV);
-  const int w = radix_sort_pairs(k0.as<unsigned>(), v0.as<unsigned>(), k1.as<unsigned>(), v1.as<unsigned>(), nV, bits_for(maxv), hist.as<unsigned>(), scr.as<unsigned>(), st);
-  unsigned* sk = w ? k1.as<unsigned>() : k0.as<unsigned>(); unsigned* sv = w ? v1.as<unsigned>() : v0.as<unsigned>();
+  Scratch s; DBuf head, idx, dense, dsegids, doff;
+  if (int rc = s.ensure(nmax, nmax + 1)) return rc;
+  SCN_ALLOC(head, nV * 4); SCN_ALLOC(idx, (nV + 1) * 4); SCN_ALLOC(dense, nV * 4); SCN_ALLOC(dsegids, nV * 4); SCN_ALLOC(doff, (nV + 1) * 8);
+  unsigned *k0 = s.k0.as<unsigned>(), *v0 = s.v0.as<unsigned>(), *k1 = s.k1.as<unsigned>(), *v1 = s.v1.as<unsigned>();
+  SCN_CUDA_TRY(cudaMemcpyAsync(k0, seg, nV * 4, cudaMemcpyHostToDevice, st));
+  k_iota<<<grid_for(nV), 256, 0, st>>>(v0, nV);
+  const int w = radix_sort_pairs(k0, v0, k1, v1, nV, bits_for(maxv), s.hist.as<unsigned>(), s.scr.as<unsigned>(), st);
+  unsigned* sk = w ? k1 : k0; unsigned* sv = w ? v1 : v0;
   k_heads<<<grid_for(nV), 256, 0, st>>>(sk, nV, head.as<unsigned>());
-  scn::exclusive_scan_u32(head.as<unsigned>(), idx.as<unsigned>(), nV, scr.as<unsigned>(), st);
+  scn::exclusive_scan_u32(head.as<unsigned>(), idx.as<unsigned>(), nV, s.scr.as<unsigned>(), st);
   k_emit_segments<<<grid_for(nV), 256, 0, st>>>(sk, sv, head.as<unsigned>(), idx.as<unsigned>(), nV, dsegids.as<unsigned>(),
                                                 doff.as<unsigned long long>(), dense.as<unsigned>());
   unsigned nS = 0;
   SCN_CUDA_TRY(cudaMemcpyAsync(&nS, idx.as<unsigned>() + nV, 4, cudaMemcpyDeviceToHost, st));
   SCN_CUDA_TRY(cudaStreamSynchronize(st));
-  uint32_t* h_ids = (uint32_t*)malloc((size_t)nS * 4); uint64_t* h_off = (uint64_t*)malloc(((size_t)nS + 1) * 8);
-  uint32_t* h_vid = (uint32_t*)malloc(nV * 4); float* h_area = want_area ? (float*)malloc((size_t)nS * 4) : nullptr;
-  auto bail = [&](int rc) { free(h_ids); free(h_off); free(h_vid); free(h_area); return rc; };
-  if (!h_ids || !h_off || !h_vid || (want_area && !h_area)) return bail(scn::fail(SCN_ERR_ARG, "scn_segs_aggregate: out of host memory"));
-  if (cudaMemcpyAsync(h_ids, dsegids.p, (size_t)nS * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-      cudaMemcpyAsync(h_off, doff.p, ((size_t)nS + 1) * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
-      cudaMemcpyAsync(h_vid, sv, nV * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess)
-    return bail(scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: download failed: %s", cudaGetErrorString(cudaGetLastError())));
+  MallocPtr<uint32_t> h_ids((uint32_t*)malloc((size_t)nS * 4)); MallocPtr<uint64_t> h_off((uint64_t*)malloc(((size_t)nS + 1) * 8));
+  MallocPtr<uint32_t> h_vid((uint32_t*)malloc(nV * 4)); MallocPtr<float> h_area(want_area ? (float*)malloc((size_t)nS * 4) : nullptr);
+  if (!h_ids || !h_off || !h_vid || (want_area && !h_area)) return scn::fail(SCN_ERR_ARG, "scn_segs_aggregate: out of host memory");
+  if (cudaMemcpyAsync(h_ids.get(), dsegids.p, (size_t)nS * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaMemcpyAsync(h_off.get(), doff.p, ((size_t)nS + 1) * 8, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaMemcpyAsync(h_vid.get(), sv, nV * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess)
+    return scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: download failed: %s", cudaGetErrorString(cudaGetLastError()));
   if (want_area) {
     DBuf dxyz, dtri, darea, dout;
-    if (!dxyz.alloc(nV * 12) || !dtri.alloc(std::max<size_t>(nF, 1) * 12) || !darea.alloc(std::max<size_t>(nF, 1) * 4) || !dout.alloc((size_t)nS * 4)) {
-      cudaGetLastError(); return bail(scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: cudaMalloc failed")); }
+    if (!dxyz.alloc(nV * 12) || !dtri.alloc(std::max<size_t>(nF, 1) * 12) || !darea.alloc(std::max<size_t>(nF, 1) * 4) || !dout.alloc((size_t)nS * 4))
+      return scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: cudaMalloc failed");
     cudaMemcpyAsync(dxyz.p, xyz, nV * 12, cudaMemcpyHostToDevice, st);
     if (nF) cudaMemcpyAsync(dtri.p, tri, nF * 12, cudaMemcpyHostToDevice, st);
-    unsigned* fk = sk == k0.as<unsigned>() ? k1.as<unsigned>() : k0.as<unsigned>();     // the buffers not holding the sorted vertex lists
-    unsigned* fv = sk == k0.as<unsigned>() ? v1.as<unsigned>() : v0.as<unsigned>();
+    unsigned* fk = sk == k0 ? k1 : k0;     // the buffers not holding the sorted vertex lists
+    unsigned* fv = sk == k0 ? v1 : v0;
     // sort faces by dense segment index; needs a second pair of buffers
     DBuf fk2, fv2;
-    if (!fk2.alloc(std::max<size_t>(nF, 1) * 4) || !fv2.alloc(std::max<size_t>(nF, 1) * 4)) { cudaGetLastError(); return bail(scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: cudaMalloc failed")); }
+    if (!fk2.alloc(std::max<size_t>(nF, 1) * 4) || !fv2.alloc(std::max<size_t>(nF, 1) * 4)) return scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: cudaMalloc failed");
     const unsigned* skey = fk; const unsigned* sfid = fv;
     if (nF) {
       k_face_keys<<<grid_for(nF), 256, 0, st>>>(dxyz.as<float>(), dtri.as<unsigned>(), nF, nV, dense.as<unsigned>(), nS, fk, fv, darea.as<float>());
-      const int w2 = radix_sort_pairs(fk, fv, fk2.as<unsigned>(), fv2.as<unsigned>(), nF, bits_for(nS), hist.as<unsigned>(), scr.as<unsigned>(), st);
+      const int w2 = radix_sort_pairs(fk, fv, fk2.as<unsigned>(), fv2.as<unsigned>(), nF, bits_for(nS), s.hist.as<unsigned>(), s.scr.as<unsigned>(), st);
       if (w2) { skey = fk2.as<unsigned>(); sfid = fv2.as<unsigned>(); }
     }
     k_segment_area<<<(unsigned)(((size_t)nS * 32 + 255) / 256), 256, 0, st>>>(skey, sfid, nF, darea.as<float>(), nS, dout.as<float>());
-    if (cudaMemcpyAsync(h_area, dout.p, (size_t)nS * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
-      return bail(scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: area pass failed: %s", cudaGetErrorString(cudaGetLastError())));
+    if (cudaMemcpyAsync(h_area.get(), dout.p, (size_t)nS * 4, cudaMemcpyDeviceToHost, st) != cudaSuccess || cudaStreamSynchronize(st) != cudaSuccess)
+      return scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: area pass failed: %s", cudaGetErrorString(cudaGetLastError()));
   }
   if (cudaStreamSynchronize(st) != cudaSuccess || cudaGetLastError() != cudaSuccess)
-    return bail(scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: kernel failed"));
-  *seg_ids_out = h_ids; *n_segs = nS; *vert_offsets = h_off; *vert_ids = h_vid; if (area_out) *area_out = h_area;
+    return scn::fail(SCN_ERR_CUDA, "scn_segs_aggregate: kernel failed");
+  *seg_ids_out = h_ids.release(); *n_segs = nS; *vert_offsets = h_off.release(); *vert_ids = h_vid.release(); if (area_out) *area_out = h_area.release();
   return SCN_OK;
 }
 
@@ -326,7 +312,7 @@ int scn_segs_objects_per_vertex(const uint32_t* seg, uint64_t nV, const uint32_t
   for (size_t i = 0; i < tab.size(); ++i) if (i + 1 == tab.size() || tab[i + 1].first != tab[i].first) { ts.push_back(tab[i].first); to.push_back(tab[i].second); }
   cudaStream_t st = 0;
   DBuf dseg, dts, dto, dobj;
-  SEGS_ALLOC(dseg, nV * 4); SEGS_ALLOC(dts, ts.size() * 4); SEGS_ALLOC(dto, ts.size() * 4); SEGS_ALLOC(dobj, nV * 4);
+  SCN_ALLOC(dseg, nV * 4); SCN_ALLOC(dts, ts.size() * 4); SCN_ALLOC(dto, ts.size() * 4); SCN_ALLOC(dobj, nV * 4);
   SCN_CUDA_TRY(cudaMemcpyAsync(dseg.p, seg, nV * 4, cudaMemcpyHostToDevice, st));
   if (!ts.empty()) { SCN_CUDA_TRY(cudaMemcpyAsync(dts.p, ts.data(), ts.size() * 4, cudaMemcpyHostToDevice, st)); SCN_CUDA_TRY(cudaMemcpyAsync(dto.p, to.data(), ts.size() * 4, cudaMemcpyHostToDevice, st)); }
   k_objects<<<grid_for(nV), 256, 0, st>>>(dseg.as<unsigned>(), nV, dts.as<unsigned>(), dto.as<unsigned>(), ts.size(), dobj.as<unsigned>());
@@ -342,8 +328,8 @@ int scn_mesh_vertex_normals(const float* xyz, uint64_t nV, const uint32_t* tri, 
   for (uint64_t c = 0; c < 3 * nF; ++c) if (tri[c] >= nV) return scn::fail(SCN_ERR_ARG, "scn_mesh_vertex_normals: face %llu references vertex %u of %llu", (unsigned long long)(c / 3), tri[c], (unsigned long long)nV);
   cudaStream_t st = 0;
   DBuf dxyz, dtri, dfn, ddeg, doff, dcur, dcsr, dscr, dn;
-  SEGS_ALLOC(dxyz, nV * 12); SEGS_ALLOC(dtri, nF * 12); SEGS_ALLOC(dfn, nF * 16); SEGS_ALLOC(ddeg, nV * 4); SEGS_ALLOC(doff, (nV + 1) * 4);
-  SEGS_ALLOC(dcur, nV * 4); SEGS_ALLOC(dcsr, nF * 12); SEGS_ALLOC(dscr, scn::scan_scratch_elems(nV) * 4); SEGS_ALLOC(dn, nV * 12);
+  SCN_ALLOC(dxyz, nV * 12); SCN_ALLOC(dtri, nF * 12); SCN_ALLOC(dfn, nF * 16); SCN_ALLOC(ddeg, nV * 4); SCN_ALLOC(doff, (nV + 1) * 4);
+  SCN_ALLOC(dcur, nV * 4); SCN_ALLOC(dcsr, nF * 12); SCN_ALLOC(dscr, scn::scan_scratch_elems(nV) * 4); SCN_ALLOC(dn, nV * 12);
   SCN_CUDA_TRY(cudaMemcpyAsync(dxyz.p, xyz, nV * 12, cudaMemcpyHostToDevice, st));
   if (nF) SCN_CUDA_TRY(cudaMemcpyAsync(dtri.p, tri, nF * 12, cudaMemcpyHostToDevice, st));
   SCN_CUDA_TRY(cudaMemsetAsync(ddeg.p, 0, nV * 4, st)); SCN_CUDA_TRY(cudaMemsetAsync(dcur.p, 0, nV * 4, st));
@@ -375,18 +361,20 @@ int scn_propagate_labels(const float* src_xyz, const float* src_normals, const u
   g.nx = (int)std::floor((mx[0] - mn[0]) * g.inv) + 1; g.ny = (int)std::floor((mx[1] - mn[1]) * g.inv) + 1; g.nz = (int)std::floor((mx[2] - mn[2]) * g.inv) + 1;
   const size_t ncell = (size_t)g.nx * g.ny * g.nz;                       // <= 101^3: cell edge >= 1 % of the largest extent
   cudaStream_t st = 0;
-  DBuf sx, sn, so, dx, dn, dout, k0, v0, k1, v1, hist, scr, cnt, cstart;
-  SEGS_ALLOC(sx, nS * 12); SEGS_ALLOC(sn, nS * 12); SEGS_ALLOC(so, nS * 4); SEGS_ALLOC(dx, nD * 12); SEGS_ALLOC(dn, nD * 12); SEGS_ALLOC(dout, nD * 4);
-  SEGS_ALLOC(k0, nS * 4); SEGS_ALLOC(v0, nS * 4); SEGS_ALLOC(k1, nS * 4); SEGS_ALLOC(v1, nS * 4); SEGS_ALLOC(hist, rs_hist_elems(nS) * 4);
-  SEGS_ALLOC(scr, scn::scan_scratch_elems(std::max(rs_hist_elems(nS), ncell + 2)) * 4); SEGS_ALLOC(cnt, (ncell + 1) * 4); SEGS_ALLOC(cstart, (ncell + 2) * 4);
+  DBuf sx, sn, so, dx, dn, dout, cnt, cstart;
+  Scratch s;
+  SCN_ALLOC(sx, nS * 12); SCN_ALLOC(sn, nS * 12); SCN_ALLOC(so, nS * 4); SCN_ALLOC(dx, nD * 12); SCN_ALLOC(dn, nD * 12); SCN_ALLOC(dout, nD * 4);
+  if (int rc = s.ensure(nS, ncell + 2)) return rc;
+  SCN_ALLOC(cnt, (ncell + 1) * 4); SCN_ALLOC(cstart, (ncell + 2) * 4);
   SCN_CUDA_TRY(cudaMemcpyAsync(sx.p, src_xyz, nS * 12, cudaMemcpyHostToDevice, st)); SCN_CUDA_TRY(cudaMemcpyAsync(sn.p, src_normals, nS * 12, cudaMemcpyHostToDevice, st));
   SCN_CUDA_TRY(cudaMemcpyAsync(so.p, src_obj, nS * 4, cudaMemcpyHostToDevice, st)); SCN_CUDA_TRY(cudaMemcpyAsync(dx.p, dst_xyz, nD * 12, cudaMemcpyHostToDevice, st));
   SCN_CUDA_TRY(cudaMemcpyAsync(dn.p, dst_normals, nD * 12, cudaMemcpyHostToDevice, st));
   SCN_CUDA_TRY(cudaMemsetAsync(cnt.p, 0, (ncell + 1) * 4, st));
-  k_cell_keys<<<grid_for(nS), 256, 0, st>>>(sx.as<float>(), so.as<unsigned>(), nS, g, k0.as<unsigned>(), v0.as<unsigned>(), cnt.as<unsigned>());
-  const int w = radix_sort_pairs(k0.as<unsigned>(), v0.as<unsigned>(), k1.as<unsigned>(), v1.as<unsigned>(), nS, bits_for((unsigned)ncell), hist.as<unsigned>(), scr.as<unsigned>(), st);
-  scn::exclusive_scan_u32(cnt.as<unsigned>(), cstart.as<unsigned>(), ncell + 1, scr.as<unsigned>(), st);
-  k_propagate<<<grid_for(nD), 256, 0, st>>>(sx.as<float>(), sn.as<float>(), so.as<unsigned>(), w ? v1.as<unsigned>() : v0.as<unsigned>(), cstart.as<unsigned>(), g,
+  unsigned* order = s.v0.as<unsigned>();
+  k_cell_keys<<<grid_for(nS), 256, 0, st>>>(sx.as<float>(), so.as<unsigned>(), nS, g, s.k0.as<unsigned>(), order, cnt.as<unsigned>());
+  sort_pass(s, order, nS, bits_for((unsigned)ncell), st);
+  scn::exclusive_scan_u32(cnt.as<unsigned>(), cstart.as<unsigned>(), ncell + 1, s.scr.as<unsigned>(), st);
+  k_propagate<<<grid_for(nD), 256, 0, st>>>(sx.as<float>(), sn.as<float>(), so.as<unsigned>(), order, cstart.as<unsigned>(), g,
                                             dx.as<float>(), dn.as<float>(), nD, max_thresh, normal_thresh, dout.as<unsigned>());
   SCN_CUDA_TRY(cudaMemcpyAsync(dst_obj_out, dout.p, nD * 4, cudaMemcpyDeviceToHost, st));
   SCN_CUDA_TRY(cudaStreamSynchronize(st));
