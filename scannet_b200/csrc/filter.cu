@@ -80,15 +80,13 @@ int launch_filter(const float* d_in, float* d_out, int W, int H, int n, float sd
 // used by run_batch (tsdf.cu) when params.depth_filter is set: u16 -> metres(-inf) -> bilateral, on the allocation stream
 int scn_filter_batch(scn_tsdf* t, int n, const uint16_t* d_depth, const BatchParams& bp, int parity, const float** out) {
   const size_t px = (size_t)t->p.width * t->p.height, K = t->p.batch_frames;
-  if (!t->filt_raw) {
-    SCN_CUDA_TRY(cudaMalloc(&t->filt_raw, 2 * K * px * 4));
-    SCN_CUDA_TRY(cudaMalloc(&t->filt_out, 2 * K * px * 4));
-  }
-  float* raw = t->filt_raw + (size_t)parity * K * px;
-  float* flt = t->filt_out + (size_t)parity * K * px;
+  if (!t->filt_raw.p) SCN_ALLOC(t->filt_raw, 2 * K * px * 4);
+  if (!t->filt_out.p) SCN_ALLOC(t->filt_out, 2 * K * px * 4);
+  float* raw = t->filt_raw.as<float>() + (size_t)parity * K * px;
+  float* flt = t->filt_out.as<float>() + (size_t)parity * K * px;
   dim3 g((unsigned)((px + 255) / 256), n);
-  k_depth_to_metres_minf<<<g, 256, 0, t->alloc_stream>>>(d_depth, bp, t->vp.depth_shift, px, raw);
-  int rc = launch_filter(raw, flt, (int)t->p.width, (int)t->p.height, n, t->p.depth_sigma_d, t->p.depth_sigma_r, t->alloc_stream);
+  k_depth_to_metres_minf<<<g, 256, 0, t->alloc_stream.get()>>>(d_depth, bp, t->vp.depth_shift, px, raw);
+  int rc = launch_filter(raw, flt, (int)t->p.width, (int)t->p.height, n, t->p.depth_sigma_d, t->p.depth_sigma_r, t->alloc_stream.get());
   if (rc) return rc;
   t->launches += 2;
   *out = flt;

@@ -194,9 +194,9 @@ extern "C" int scn_tsdf_extract_mesh(scn_tsdf* t, float** xyz, uint8_t** rgb, ui
   SCN_CUDA_TRY(cudaSetDevice(t->device));
   SCN_CUDA_TRY(cudaStreamSynchronize(t->stream));
   cudaStream_t st = t->stream;
-  unsigned long long cnt[C_COUNT];
-  SCN_CUDA_TRY(cudaMemcpy(cnt, t->tb.counters, sizeof(cnt), cudaMemcpyDeviceToHost));
-  const size_t N = (size_t)std::min<unsigned long long>(cnt[C_HEAP], t->tb.max_blocks);
+  Counters cnt;
+  { int rc = read_counters(t, cnt); if (rc) return rc; }
+  const size_t N = (size_t)cnt.blocks;
   *n_verts = *n_faces = 0; *xyz = nullptr; *tri = nullptr; if (rgb) *rgb = nullptr;
   if (N == 0) { *xyz = (float*)malloc(16); *tri = (uint32_t*)malloc(16); if (rgb) *rgb = (uint8_t*)malloc(16); return SCN_OK; }
   // deterministic block order: ascending packed key

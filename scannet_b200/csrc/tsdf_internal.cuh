@@ -1,6 +1,7 @@
 // Internal declarations shared by tsdf.cu (fusion) and mc.cu (meshing): device tables, key packing, hash,
 // and the host-side handle.  Not part of the public ABI.
 #pragma once
+#include <algorithm>
 #include <vector>
 
 #include "scn_common.h"
@@ -62,7 +63,7 @@ __device__ __forceinline__ unsigned long long pack_key(int x, int y, int z) {
   return (unsigned long long)(unsigned)(x + kKeyBias) | ((unsigned long long)(unsigned)(y + kKeyBias) << 21) |
          ((unsigned long long)(unsigned)(z + kKeyBias) << 42);
 }
-__device__ __forceinline__ void unpack_key(unsigned long long k, int& x, int& y, int& z) {
+__host__ __device__ __forceinline__ void unpack_key(unsigned long long k, int& x, int& y, int& z) {
   x = (int)(k & 0x1FFFFF) - kKeyBias;
   y = (int)((k >> 21) & 0x1FFFFF) - kKeyBias;
   z = (int)((k >> 42) & 0x1FFFFF) - kKeyBias;
@@ -99,34 +100,48 @@ struct scn_tsdf {
   int device = 0;
   int sm_count = 132;
   scn_tsdf_detail::VolParams vp{};
-  scn_tsdf_detail::Tables tb{};
+  scn_tsdf_detail::Tables tb{};                  // the buffers below as the kernels see them (filled once, after allocation)
   uint64_t cap = 0;
-  float* dm = nullptr;
-  float* depth_lut = nullptr;       // raw u16 depth -> metres or NaN (spec step A + range test), 65536 entries
-  unsigned* rgbx = nullptr;        // colour of the current batches repacked to one word per pixel (2 parities), allocated on first use
-  uint16_t* d_depth[2] = {nullptr, nullptr};     // H2D staging, double buffered
-  uint8_t* d_rgb[2] = {nullptr, nullptr};
-  uint16_t* h_depth[2] = {nullptr, nullptr};     // pinned bounce buffers (pageable callers)
-  uint8_t* h_rgb[2] = {nullptr, nullptr};
-  cudaStream_t stream = nullptr, copy_stream = nullptr, alloc_stream = nullptr;
-  cudaEvent_t ev_alloc_done[2]{}, ev_integ_done[2]{}, ev_input{};
+  scn::DBuf keys, vals, block_keys, counters, heap;
+  scn::DBuf mask_base, list_base;                // 2 x cap, 2 x max_blocks: one set per batch parity
+  scn::DBuf dm;
+  scn::DBuf depth_lut;                           // raw u16 depth -> metres or NaN (spec step A + range test), 65536 entries
+  scn::DBuf rgbx;                                // colour of the current batches repacked to one word per pixel (2 parities), allocated on first use
+  scn::DBuf d_depth[2], d_rgb[2];                // H2D staging, double buffered
+  scn::PinnedPtr<uint16_t> h_depth[2];           // pinned bounce buffers (pageable callers)
+  scn::PinnedPtr<uint8_t> h_rgb[2];
+  cudaStream_t stream = nullptr;                 // the caller's stream (scn_tsdf_set_stream), not owned
+  scn::StreamPtr copy_stream, alloc_stream;
+  scn::EventPtr ev_alloc_done[2], ev_integ_done[2], ev_input;
   bool parity_used[2] = {false, false};
-  unsigned int* mask_base = nullptr; unsigned int* list_base = nullptr;   // 2 x cap, 2 x max_blocks
-  int alloc_group = 4;                           // frames of a batch walked by one k_alloc CTA (shared-memory key map reuse)
-  int reserve_ctas = 0;                          // integrate CTAs per SM left free for the next batch's k_alloc (measured: 0 is best, SCN_TSDF_RESERVE)
-  bool own_stream = false;
   bool heap_zeroed = false;                      // the whole heap has been cleared once; later resets clear only the used prefix
-  cudaEvent_t ev_copied[2]{}, ev_consumed[2]{};
+  scn::EventPtr ev_copied[2], ev_consumed[2];
   bool buf_used[2] = {false, false};
   int parity = 0;
   uint64_t frames_integrated = 0, frames_skipped = 0, frame_bytes = 0, launches = 0;
   uint64_t chunk_seq = 0;
   bool profile = false;
-  std::vector<cudaEvent_t> prof_events;   // 4 per batch: around k_alloc (allocation stream), around the integrate kernel
+  std::vector<scn::EventPtr> prof_events;        // 4 per batch: around k_alloc (allocation stream), around the integrate kernel
   size_t prof_used = 0;
-  float* filt_raw = nullptr; float* filt_out = nullptr;   // bilateral pre-filter scratch: 2 parities x K frames each (lazy)
+  scn::DBuf filt_raw, filt_out;                  // bilateral pre-filter scratch: 2 parities x K frames each (lazy)
   float mc_thresh_factor = 10.0f;         // s_SDFMarchingCubeThreshFactor (zParametersScanNet.txt:48)
 };
+
+namespace scn_tsdf_detail {
+
+// Host copy of the device counters; the caller first synchronises the streams that write them.  `blocks` is the heap
+// count clamped to max_blocks: the allocator keeps counting past an exhausted heap.
+struct Counters {
+  unsigned long long c[C_COUNT];
+  uint64_t blocks;
+};
+inline int read_counters(const scn_tsdf* t, Counters& out) {
+  SCN_CUDA_TRY(cudaMemcpy(out.c, t->tb.counters, sizeof(out.c), cudaMemcpyDeviceToHost));
+  out.blocks = std::min<uint64_t>(out.c[C_HEAP], t->tb.max_blocks);
+  return SCN_OK;
+}
+
+}  // namespace scn_tsdf_detail
 
 // filter.cu: u16 -> metres (-inf invalid) -> bilateral filter for the n frames of a batch, on the allocation stream
 int scn_filter_batch(scn_tsdf* t, int n, const uint16_t* d_depth, const scn_tsdf_detail::BatchParams& bp, int parity, const float** out);

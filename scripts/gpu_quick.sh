@@ -5,15 +5,3 @@ OUT=gpurun_out; mkdir -p $OUT
 timeout 600 python -m pytest tests/test_tsdf_gpu.py -x -q 2>&1 | tail -5
 for B in ${BATCHES:-8 16}; do timeout 600 python bench.py --no-cpu --no-seg --batch $B > $OUT/bench_q${B}_$TAG.json 2>$OUT/bench_q${B}_$TAG.err; python -c "
 import json,sys; d=json.load(open('$OUT/bench_q${B}_$TAG.json')); r=d['roofline']; print('batch $B value', round(d['value']), 'e2e', round(d['e2e']['value']), 'integ_ms/launch', round(r['avg_launch_ms'],4), 'alloc_total_ms', round(r['alloc_kernel_ms_total'],2), 'integ_total_ms', round(r['integrate_kernel_ms_total'],2), 'ms_per_step', round(d['ms_per_step'],3))" || tail -3 $OUT/bench_q${B}_$TAG.err; done
-
-if [ -n "$NCU_ALLOC" ]; then
-  for G in $NCU_ALLOC; do SCN_TSDF_ALLOC_GROUP=$G timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -k regex:k_ -c 60 --csv --log-file $OUT/l_$G.csv python bench.py --steps 2 --warmup 1 --frames-per-step 48 --no-cpu --no-seg --batch ${NCU_BATCH:-8} >/dev/null 2>&1; python - <<PY
-import csv
-rows=[r for r in csv.DictReader(l for l in open("$OUT/l_$G.csv") if l.startswith('"'))]
-from collections import defaultdict
-d=defaultdict(list)
-for r in rows: d[r["Kernel Name"].split("(")[0][-24:]].append(float(r["Metric Value"]))
-print("group $G batch ${NCU_BATCH:-8}:", {k:(len(v), round(sum(v)/len(v)/1e3,1)) for k,v in d.items()})
-PY
-  done
-fi

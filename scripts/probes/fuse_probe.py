@@ -1,5 +1,4 @@
-"""Where the time of one file -> TSDF scene goes (scn_fuse_scene reports) against the decode chunk size and the number of
-integrate CTAs per SM left free for the decoders.
+"""Where the time of one file -> TSDF scene goes (scn_fuse_scene reports) against the decode chunk size.
 Usage: python scripts/probes/fuse_probe.py [frames] [color 0|1] [quick] > gpurun_out/fuse_probe.json   (the JSON goes to stdout)"""
 import json
 import os
@@ -23,15 +22,14 @@ with tempfile.TemporaryDirectory() as d:
     p = os.path.join(d, "scene.sens")
     bench.make_sens_file(p, n, 100, dev, with_color=color)
     over = dict(max_blocks=1 << 22, hash_slots=1 << 24) if color else {}
-    sweep = (("1024", "0"), ("1024", "3"), ("512", "0"), ("2048", "0")) if len(sys.argv) <= 3 else (("1024", "0"),)
-    for chunk, reserve in sweep:
+    sweep = ("1024", "512", "2048") if len(sys.argv) <= 3 else ("1024",)
+    for chunk in sweep:
         os.environ["SCN_FUSE_CHUNK"] = chunk
-        os.environ["SCN_TSDF_RESERVE"] = reserve
         runs = []
         for rep_i in range(2 if len(sys.argv) <= 3 else 4):
             t0 = time.perf_counter()
             rep = sfuse.fuse_scene(p, None, decode_mode="gpu", device=0, **over)
             rep["wall_s"] = time.perf_counter() - t0
             runs.append({k: round(rep[k], 4) for k in keys})
-        out[f"chunk_{chunk}_reserve_{reserve}"] = runs
+        out[f"chunk_{chunk}"] = runs
 os.write(bench._REAL_STDOUT, (json.dumps(out, indent=1) + "\n").encode())

@@ -248,10 +248,8 @@ def test_depth_shift(built):
 
 # ---- scheduling -------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("batch", [1, 2, 7, 32])
-@pytest.mark.parametrize("env", [("SCN_TSDF_ALLOC_GROUP", "1"), ("SCN_TSDF_ALLOC_GROUP", "3"), ("SCN_TSDF_ALLOC_GROUP", "5"),
-                                 ("SCN_TSDF_ALLOC_GROUP", "32"), ("SCN_TSDF_RESERVE", "2")])
-def test_frame_grouping_and_reserve(built, monkeypatch, env, batch):
-    monkeypatch.setenv(*env)
+def test_frame_grouping(built, batch):
+    """one k_alloc CTA walks 4 frames of a batch: batches below one group, a partial last group (7 = 4 + 3) and 8 groups"""
     D, C, P, K = room(35, loop=200)
     compare(prm(64, 48, batch_frames=batch), D, None, P, K, mesh=batch == 7)
 
