@@ -34,6 +34,7 @@ oracle:
 	$(MAKE) -C oracle all
 	$(MAKE) -C oracle -f meshclean.mk all
 	$(MAKE) -C oracle -f meshsimplify.mk all
+	$(MAKE) -C oracle -f freespace.mk all
 
 $(OBJDIR) $(LIBDIR) $(BINDIR):
 	mkdir -p $@

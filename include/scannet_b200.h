@@ -437,6 +437,69 @@ int  scn_mesh_simplify(const float* xyz, const uint8_t* rgb, uint64_t n_verts, c
  * Without -s the simplify.mlx defaults apply; without `-m vc` the output carries no colour (white). */
 int  scn_meshsimplify_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Free-space occupancy grid (DESIGN.md §6h): the `freespace` stage, `FreeSpace.exe <id>.sens` -> `<id>.grid`
+ * (Server/config/scan_stages.json:43-47, Server/scan_processor.py:150-152).  FreeSpace.exe is not in the reference tree, so the
+ * numerics are this repository's own "free-space spec v1" (parity unpinned).  Every voxel of a dense lattice box counts the
+ * frames that saw it free (in front of the measured surface) and occupied (inside the band around it); the label is
+ * 0 unknown, 1 free, 2 occupied.  Counting runs on the GPU; there is no CPU fallback.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct scn_freespace scn_freespace;
+typedef struct {
+  float    voxel_size;                /* vs, metres (0.05); voxel g has its centre at g*vs                              */
+  float    band_base, band_scale;     /* band(d) = fma(band_scale, d, band_base): 0.05 m + 0.01 per metre of depth       */
+  float    depth_min, depth_max;      /* valid depth range (0.1 / 6.0 m, zParametersScanNet.txt:34-35)                   */
+  float    max_distance;              /* observations end here (4.0 m, zParametersScanNet.txt:51)                        */
+  uint64_t max_voxels;                /* capacity of the counted box (2^28 = 2 GiB of counters); larger boxes are refused */
+} scn_freespace_params;
+typedef struct scn_freespace_report {
+  uint64_t frames_used, frames_skipped_pose;   /* frames classified; frames without a pose (cam2world[0] == -inf), never decoded */
+  uint64_t envelope_dims[3], output_dims[3];   /* the counted box; the cropped box of labelled voxels (0 when none) */
+  int32_t  envelope_lo[3], output_lo[3];
+  uint64_t voxels_free, voxels_occupied, voxels_unknown;   /* labels of the output box */
+  uint64_t pairs_classified, pairs_culled;     /* (8^3 brick, frame) pairs the classify kernel ran / skipped by the frustum test */
+  double   decode_s;                           /* depth decode (GPU inflate or upload), host clock around each call */
+  double   classify_ms;                        /* classify kernels, CUDA events */
+  double   crop_ms;                            /* label + crop + download, host clock */
+  double   write_s, total_s;                   /* .grid write; the whole call incl. opening the file */
+} scn_freespace_report_t;
+void   scn_freespace_default_params(scn_freespace_params* p);
+size_t scn_freespace_report_sizeof(void);
+/* The lattice box that holds every voxel the frames can observe, from the poses alone (host only, binary64): the camera centres
+ * of the frames with a pose, widened by (max_distance + band(max_distance)) * |(1, (corner - c) / f)| over the image corners
+ * +-1 px, plus one voxel, rounded outward.  No frame with a pose: dims 0.  SCN_ERR_ARG: invalid parameters, fx or fy <= 0, a
+ * box beyond +-2^23 voxels. */
+int  scn_freespace_envelope(const float* cam2world, uint32_t n, const float K[16], uint32_t width, uint32_t height,
+                            const scn_freespace_params* p, int32_t lo[3], uint64_t dims[3]);
+/* Counts over the box lo .. lo+dims-1 for width x height depth frames.  SCN_ERR_ARG: vs <= 0 or NaN, a band term negative or
+ * NaN, depth_min >= depth_max, max_distance <= 0, depth_shift <= 0, frames of 0 or more than 2^24 pixels, a box beyond
+ * +-2^23 voxels; SCN_ERR_CAPACITY: a box of more than max_voxels voxels (never truncated). */
+int  scn_freespace_create(const scn_freespace_params* p, uint32_t width, uint32_t height, float depth_shift, const int32_t lo[3],
+                          const uint64_t dims[3], int device, scn_freespace** out);
+void scn_freespace_destroy(scn_freespace* h);
+/* n frames, depth n*W*H u16 on the HOST (_integrate) or in DEVICE memory (_integrate_device); poses n*16 row-major cam2world and
+ * K (4x4 depth intrinsic as in a .sens header) on the host.  Frames whose pose is invalid (cam2world[0] == -inf) are skipped
+ * and their depth is never read.  Counts commute: frame order and the split into calls do not change them.  Returns when the
+ * frames are counted.  Host frames travel in one copy per batch on the handle's stream; device frames must be complete when
+ * _integrate_device is called (the work that wrote them has finished, as when scn_inflate_batch_device has returned). */
+int  scn_freespace_integrate(scn_freespace* h, uint32_t n, const uint16_t* depth, const float* cam2world, const float K[16]);
+int  scn_freespace_integrate_device(scn_freespace* h, uint32_t n, const uint16_t* d_depth, const float* cam2world, const float K[16]);
+/* The smallest box holding every labelled voxel: labels (u8, x fastest), and optionally the two counts (u32), malloc'ed
+ * (scn_free); n_free / n_occ may be NULL.  Empty result: dims 0, lo 0, NULL arrays. */
+int  scn_freespace_download(scn_freespace* h, int32_t lo_out[3], uint64_t dims_out[3], uint8_t** labels, uint32_t** n_free,
+                            uint32_t** n_occ);
+/* What the handle did so far (frames, box, pairs, classify time; output box, label counts and crop time of the last download) */
+int  scn_freespace_handle_report(const scn_freespace* h, scn_freespace_report_t* report);
+/* .grid file (DESIGN.md §6h): "SCNGRID\0", u32 version 1, f32 vs, u64 dims[3], i32 lo[3], u8 labels x fastest */
+int  scn_freespace_save_grid(const char* path, float voxel_size, const int32_t lo[3], const uint64_t dims[3], const uint8_t* labels);
+/* The stage: every frame of the .sens with a pose (depth inflated on the GPU) -> envelope -> counts -> labels -> out_grid
+ * (NULL: no file).  width, height and depth_shift come from the stream.  report may be NULL. */
+int  scn_freespace_scene(const char* sens_path, const char* out_grid, const scn_freespace_params* p, int device,
+                         scn_freespace_report_t* report);
+/* `freespace [params.txt] <file.sens> [out.grid] [--voxel V]`: writes <base>.grid beside the input unless an output is given.
+ * params.txt (scn_tsdf_params_from_file) sets the depth range and max_distance; --voxel V sets voxel_size = band_base = V. */
+int  scn_freespace_main(int argc, const char** argv);
+
 #ifdef __cplusplus
 }
 #endif

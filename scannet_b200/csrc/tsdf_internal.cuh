@@ -2,6 +2,7 @@
 // and the host-side handle.  Not part of the public ABI.
 #pragma once
 #include <algorithm>
+#include <cmath>
 #include <vector>
 
 #include "scn_common.h"
@@ -91,6 +92,35 @@ __device__ __forceinline__ int lookup_block(const Tables& tb, int x, int y, int 
     slot = (slot + 1) & tb.cap_mask;
   }
   return -1;
+}
+
+// ------------------------------------------------------------------------------ host (shared with freespace.cu)
+// Per-frame constants of spec step C (TSDF §3, free space §6h): every product and sum is one binary32 operation in the
+// oracles' order (volatile keeps the host compiler from reassociating or widening).
+inline void make_frame_params(float vs, const float* T, const float* K, int src, bool has_rgb, FrameParams& fp) {
+  for (int i = 0; i < 12; ++i) fp.T[i] = T[i];
+  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j) fp.Rt[3 * i + j] = T[4 * j + i];
+  for (int i = 0; i < 3; ++i) {
+    volatile float a = fp.Rt[3 * i + 0] * T[3];
+    volatile float b = fp.Rt[3 * i + 1] * T[7];
+    volatile float c = fp.Rt[3 * i + 2] * T[11];
+    volatile float ab = a + b;
+    fp.tinv[i] = -(ab + c);
+  }
+  for (int i = 0; i < 9; ++i) { volatile float v = fp.Rt[i] * vs; fp.Avs[i] = v; }
+  fp.fx = K[0]; fp.cx = K[2]; fp.fy = K[5]; fp.cy = K[6];
+  { volatile float a = 1.0f / fp.fx; volatile float b = 1.0f / fp.fy; fp.ifx = a; fp.ify = b; }
+  fp.src = src; fp.has_rgb = has_rgb ? 1 : 0;
+}
+
+// Spec step A as a table: raw u16 -> metres (IEEE division, as the oracles) or NaN when outside [depth_min, depth_max]
+inline void make_depth_lut(float depth_shift, float depth_min, float depth_max, std::vector<float>& lut) {
+  lut.resize(65536);
+  for (int r = 0; r < 65536; ++r) {
+    volatile float q = r == 0 ? 0.0f : (float)r / depth_shift;
+    const float m = q;
+    lut[r] = (m >= depth_min && m <= depth_max) ? m : NAN;
+  }
 }
 
 }  // namespace scn_tsdf_detail
