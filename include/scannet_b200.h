@@ -313,7 +313,8 @@ int  scn_inflate_host(const uint8_t* src, size_t n, uint8_t* out, size_t cap, si
  * Scene fusion driver: .sens -> hashed TSDF -> (optionally) marching cubes -> <out>.ply — the contract of the reference's
  * external reconstruction stage (Server/scan_processor.py:27-35,123-138), one scene per GPU (Server/process.py:75 runs one
  * scan per GPU at a time; SURVEY.md §8e).  decode_mode: NULL = automatic, "gpu" = compressed payloads decoded in HBM,
- * "host" = host thread pool.
+ * "host" = host thread pool.  A failed scene returns the code of the first call that failed (e.g. SCN_ERR_CAPACITY for a full
+ * voxel heap), its text prefixed by the .sens path.
  * ------------------------------------------------------------------------------------------------------------------ */
 typedef struct scn_fuse_report {
   int32_t  status;                 /* 0 or the error code of this scene (scn_fuse_many) */

@@ -2,11 +2,9 @@
 //   <exe> <file.sens>                                   (Server/scan_processor.py:150-152, Server/config/scan_stages.json:43-47)
 //   <exe> [params.txt] <file.sens> [out.grid] [--voxel V]
 // Reads every pose of the .sens stream, derives the lattice box the frames can observe, inflates the depth of the frames that
-// have a pose on the GPU (scn_inflate_batch_device) chunk by chunk, counts free / occupied observations per voxel
+// have a pose on the GPU (scn::sens_depth_to_device) chunk by chunk, counts free / occupied observations per voxel
 // (scn_freespace_integrate_device), crops to the labelled voxels and writes `<base>.grid`.
 #include <algorithm>
-#include <chrono>
-#include <cmath>
 #include <cstdio>
 #include <cstring>
 #include <string>
@@ -16,15 +14,8 @@
 
 namespace {
 
-double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-constexpr uint32_t kChunk = 1024;            // frames decoded per scn_inflate_batch_device call
-
-// owners of the C-ABI resources the driver holds
-struct Sens { scn_sens* s = nullptr; ~Sens() { scn_sens_close(s); } };
-struct Handle { scn_freespace* h = nullptr; ~Handle() { scn_freespace_destroy(h); } };
-struct DevBuf { void* p = nullptr; ~DevBuf() { scn_device_free(p); } };
-template <class T> struct Owned { T* p = nullptr; ~Owned() { scn_free(p); } };
+using scn::now_s;
+constexpr uint32_t kChunk = 1024;            // frames decoded per scn::sens_depth_to_device call
 
 }  // namespace
 
@@ -53,70 +44,51 @@ int scn_freespace_scene(const char* sens_path, const char* out_grid, const scn_f
                         scn_freespace_report_t* report) {
   if (!sens_path || !params) return scn::fail(SCN_ERR_ARG, "null argument");
   const double t_begin = now_s();
-  Sens s;
-  if (int rc = scn_sens_open(sens_path, &s.s)) return rc;
+  scn_sens* sp = nullptr;
+  if (int rc = scn_sens_open(sens_path, &sp)) return rc;
+  const scn::SensPtr s(sp);
   scn_sens_info_t in;
-  if (int rc = scn_sens_info(s.s, &in)) return rc;
+  if (int rc = scn_sens_info(s.get(), &in)) return rc;
   if (in.depth_compression != 0 && in.depth_compression != 1)
     return scn::fail(SCN_ERR_UNSUPPORTED, "%s: depth compression %d (only raw and zlib u16 are decoded)", sens_path, in.depth_compression);
-  // 1. every pose (no decode)
-  std::vector<float> poses((size_t)in.n_frames * 16);
-  for (uint64_t f = 0; f < in.n_frames; ++f)
-    if (int rc = scn_sens_frame_meta(s.s, f, &poses[f * 16], nullptr, nullptr, nullptr, nullptr)) return rc;   // never a zero pose taken as valid
+  // 1. the frames that have a pose, and their poses (no decode)
+  scn::PosedFrames plan;
+  if (int rc = scn::posed_frames(s.get(), 0, in.n_frames, plan)) return rc;
+  const uint32_t n_posed = (uint32_t)plan.frames.size();
   // 2. the envelope, the handle
   int32_t lo[3]; uint64_t dims[3];
-  if (int rc = scn_freespace_envelope(poses.data(), (uint32_t)in.n_frames, in.depth_intrinsic, in.depth_width, in.depth_height, params, lo, dims)) return rc;
-  Handle h;
-  if (int rc = scn_freespace_create(params, in.depth_width, in.depth_height, in.depth_shift, lo, dims, device, &h.h)) return rc;
-  // 3. per chunk: the frames with a pose, compacted (a frame without one is never decoded: sensorData.h:382), decoded into
-  //    device memory, counted
+  if (int rc = scn_freespace_envelope(plan.poses.data(), n_posed, in.depth_intrinsic, in.depth_width, in.depth_height, params, lo, dims)) return rc;
+  scn_freespace* hp = nullptr;
+  if (int rc = scn_freespace_create(params, in.depth_width, in.depth_height, in.depth_shift, lo, dims, device, &hp)) return rc;
+  const scn::FreespacePtr h(hp);
+  // 3. those frames chunk by chunk: decoded into device memory, counted
   const size_t px = (size_t)in.depth_width * in.depth_height;
-  DevBuf d_depth;
-  void* stream = nullptr;
+  scn::HandleStreamPtr stream;
+  if (int rc = scn::create(stream)) return rc;
+  const scn::DevicePtr<uint16_t> d_depth(n_posed ? (uint16_t*)scn_device_alloc((size_t)kChunk * px * 2) : nullptr);
+  if (n_posed && !d_depth)
+    return scn::fail(SCN_ERR_CUDA, "cannot allocate %zu bytes of depth frames", (size_t)kChunk * px * 2);
   double decode_s = 0;
-  std::vector<const uint8_t*> src; std::vector<uint64_t> len; std::vector<float> cp;
-  int rc = 0;
-  if (scn_stream_create(&stream)) return SCN_ERR_CUDA;
-  for (uint64_t f0 = 0; f0 < in.n_frames && !rc; f0 += kChunk) {
-    const uint64_t f1 = std::min<uint64_t>(in.n_frames, f0 + kChunk);
-    src.clear(); len.clear(); cp.clear();
-    for (uint64_t f = f0; f < f1; ++f) {
-      if (poses[f * 16] == -INFINITY) continue;
-      const uint8_t* cpay = nullptr; const uint8_t* dpay = nullptr; uint64_t db = 0;
-      if ((rc = scn_sens_frame_payload(s.s, f, &cpay, &dpay)) || (rc = scn_sens_frame_meta(s.s, f, nullptr, nullptr, nullptr, nullptr, &db))) break;
-      src.push_back(dpay); len.push_back(db);
-      cp.insert(cp.end(), &poses[f * 16], &poses[f * 16] + 16);
-    }
-    const uint32_t n = (uint32_t)src.size();
-    if (rc) break;
-    if (!n) continue;
-    if (!d_depth.p && !(d_depth.p = scn_device_alloc((size_t)kChunk * px * 2))) { rc = scn::fail(SCN_ERR_CUDA, "cannot allocate %zu bytes of depth frames", (size_t)kChunk * px * 2); break; }
+  for (uint32_t i0 = 0; i0 < n_posed; i0 += kChunk) {
+    const uint32_t n = std::min(kChunk, n_posed - i0);
     const double td0 = now_s();
-    if (in.depth_compression == 1) {
-      rc = scn_inflate_batch_device(src.data(), len.data(), n, (uint64_t)px * 2, d_depth.p, stream);
-    } else {
-      for (uint32_t i = 0; i < n && !rc; ++i) {
-        if (len[i] < px * 2) { rc = scn::fail(SCN_ERR_FORMAT, "%s: raw depth payload of %llu bytes, need %zu", sens_path, (unsigned long long)len[i], px * 2); break; }
-        rc = scn_memcpy_h2d((uint16_t*)d_depth.p + (size_t)i * px, src[i], px * 2, stream);
-      }
-    }
+    if (int rc = scn::sens_depth_to_device(s.get(), &plan.frames[i0], n, d_depth.get(), stream.get())) return rc;
     decode_s += now_s() - td0;
-    if (!rc) rc = scn_freespace_integrate_device(h.h, n, (const uint16_t*)d_depth.p, cp.data(), in.depth_intrinsic);
+    if (int rc = scn_freespace_integrate_device(h.get(), n, d_depth.get(), &plan.poses[(size_t)i0 * 16], in.depth_intrinsic)) return rc;
   }
-  scn_stream_destroy(stream);
-  if (rc) return rc;
   // 4. labels of the crop box, the file
   int32_t olo[3]; uint64_t od[3];
-  Owned<uint8_t> labels;
-  if (int r = scn_freespace_download(h.h, olo, od, &labels.p, nullptr, nullptr)) return r;
+  uint8_t* lp = nullptr;
+  if (int r = scn_freespace_download(h.get(), olo, od, &lp, nullptr, nullptr)) return r;
+  const scn::MallocPtr<uint8_t> labels(lp);
   double write_s = 0;
   if (out_grid) {
     const double tw0 = now_s();
-    if (int r = scn_freespace_save_grid(out_grid, params->voxel_size, olo, od, labels.p)) return r;
+    if (int r = scn_freespace_save_grid(out_grid, params->voxel_size, olo, od, labels.get())) return r;
     write_s = now_s() - tw0;
   }
   scn_freespace_report_t rep;
-  if (int r = scn_freespace_handle_report(h.h, &rep)) return r;
+  if (int r = scn_freespace_handle_report(h.get(), &rep)) return r;
   rep.frames_skipped_pose = in.n_frames - rep.frames_used;
   rep.decode_s = decode_s; rep.write_s = write_s;
   rep.total_s = now_s() - t_begin;

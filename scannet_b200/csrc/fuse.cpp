@@ -12,7 +12,6 @@
 // integration, so no raw frame crosses PCIe or touches a host core.  "host" (SCN_FUSE_DECODE=host; automatic for PNG / raw
 // colour): a host thread pool inflates / decodes one chunk ahead and the frames are handed over in pinned memory.
 #include <atomic>
-#include <chrono>
 #include <condition_variable>
 #include <functional>
 #include <memory>
@@ -55,9 +54,17 @@ class Pool {
   const std::function<void()>* fn_ = nullptr; unsigned pending_ = 0; unsigned long gen_ = 0; bool stop_ = false;
 };
 
-struct Chunk { uint16_t* depth = nullptr; uint8_t* rgb = nullptr; std::vector<float> poses; uint32_t n = 0; int rc = 0; std::string err; };
+struct Chunk { scn::PinnedPtr<uint16_t> depth; scn::PinnedPtr<uint8_t> rgb; std::vector<float> poses; uint32_t n = 0; };
 
-double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+// The first call of a scene that failed, on whichever thread: its code, and its text, read on that thread (scn_last_error is
+// per thread).
+struct FirstFailure {
+  std::atomic<int> rc{0}; std::mutex m; std::string err;
+  void set(int code) { std::lock_guard<std::mutex> l(m); if (!rc.load()) { err = scn_last_error(); rc.store(code); } }
+  explicit operator bool() const { return rc.load() != 0; }
+};
+
+using scn::now_s;
 
 // colour pixel for every depth pixel: K_c * K_d^-1 * (x, y, 1), nearest (sensorData.h:1577-1586 with identity extrinsics)
 void build_color_lut(const scn_sens_info_t& in, std::vector<int32_t>& lut) {
@@ -72,31 +79,24 @@ void build_color_lut(const scn_sens_info_t& in, std::vector<int32_t>& lut) {
   }
 }
 
-void decode_chunk(const scn_sens* s, const scn_sens_info_t& in, const std::vector<int32_t>& lut, bool use_color, uint64_t f0, uint32_t n, Chunk& c, Pool& pool) {
+void decode_chunk(const scn_sens* s, const scn_sens_info_t& in, const std::vector<int32_t>& lut, bool use_color, uint64_t f0, uint32_t n, Chunk& c, Pool& pool,
+                  FirstFailure& fail) {
   const size_t px = (size_t)in.depth_width * in.depth_height;
-  c.n = n; c.rc = 0; c.poses.assign((size_t)n * 16, 0.f);
-  std::atomic<uint32_t> next{0}; std::atomic<int> rc{0};
-  std::mutex err_m;
-  auto work = [&]() {
+  c.n = n; c.poses.assign((size_t)n * 16, 0.f);
+  std::atomic<uint32_t> next{0};
+  pool.run([&]() {
     static thread_local std::vector<uint8_t> col;                               // kept per pool thread: no 1-4 MB allocation per chunk
     col.resize(use_color ? (size_t)in.color_width * in.color_height * 3 : 0);
-    for (;;) {
-      const uint32_t i = next.fetch_add(1);
-      if (i >= n || rc.load()) break;
-      scn_sens_frame_meta(s, f0 + i, &c.poses[(size_t)i * 16], nullptr, nullptr, nullptr, nullptr);
-      if (c.poses[(size_t)i * 16] == -INFINITY) continue;                        // skipped by the integrator anyway
-      int r = scn_sens_frame_depth_u16(s, f0 + i, c.depth + (size_t)i * px);
-      if (!r && use_color) {
-        r = scn_sens_frame_color_rgb8(s, f0 + i, col.data());
-        if (!r) { uint8_t* o = c.rgb + (size_t)i * px * 3;
-          for (size_t p = 0; p < px; ++p) { const int32_t q = lut[p]; if (q >= 0) { o[3 * p] = col[3 * q]; o[3 * p + 1] = col[3 * q + 1]; o[3 * p + 2] = col[3 * q + 2]; } else o[3 * p] = o[3 * p + 1] = o[3 * p + 2] = 0; } }
+    for (uint32_t i; (i = next.fetch_add(1)) < n && !fail;) {
+      float* T = &c.poses[(size_t)i * 16];
+      int r = scn_sens_frame_meta(s, f0 + i, T, nullptr, nullptr, nullptr, nullptr);
+      if (!r && T[0] != -INFINITY) {                                             // a frame without a pose is skipped by the integrator
+        r = scn_sens_frame_depth_u16(s, f0 + i, c.depth.get() + (size_t)i * px);
+        if (!r && use_color) r = scn::sens_color_to_depth(s, f0 + i, lut.data(), px, col.data(), c.rgb.get() + (size_t)i * px * 3);
       }
-      // the error text is thread-local: capture it on the worker that failed
-      if (r) { std::lock_guard<std::mutex> l(err_m); if (!rc.load()) { c.err = scn_last_error(); rc.store(r); } }
+      if (r) fail.set(r);
     }
-  };
-  pool.run(work);
-  c.rc = rc.load();
+  });
 }
 
 // ---- one scene on one GPU ------------------------------------------------------------------------------------------------------
@@ -136,11 +136,13 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
   const double t_begin = now_s();
   if (scn_set_device(job.device)) return SCN_ERR_CUDA;
   std::thread warm([dev = job.device]() { scn_set_device(dev); scn_cuda_warmup(); });          // context creation overlaps reading the .sens file
-  scn_sens* s = nullptr;
-  const int open_rc = scn_sens_open(job.sens_path.c_str(), &s);
+  scn_sens* sp = nullptr;
+  const int open_rc = scn_sens_open(job.sens_path.c_str(), &sp);
   const std::string open_err = open_rc ? scn_last_error() : "";
   warm.join();
   if (open_rc) return scn::fail(open_rc, "%s", open_err.c_str());
+  scn::SensPtr sens(sp);
+  const scn_sens* s = sens.get();
   scn_sens_info_t in; scn_sens_info(s, &in);
   scn_tsdf_params p = job.params;
   p.width = in.depth_width; p.height = in.depth_height; p.depth_shift = in.depth_shift;   // integrate at the stream's depth resolution
@@ -153,11 +155,11 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
   scn::StagePool<VolSlot>::Lease vs(vol_pool());
   if (vs->vol && !memcmp(&vs->p, &p, sizeof(p))) {                                     // same volume layout as the previous scene on this GPU
     vol = vs->vol;
-    if (scn_tsdf_reset(vol)) { const std::string e = scn_last_error(); vs->release(); scn_sens_close(s); return scn::fail(SCN_ERR_CUDA, "%s", e.c_str()); }
+    if (int r = scn_tsdf_reset(vol)) { const std::string e = scn_last_error(); vs->release(); return scn::fail(r, "%s: %s", job.sens_path.c_str(), e.c_str()); }
     rep.volume_reused = 1;
   } else {
     vs->release();
-    if (scn_tsdf_create(&p, job.device, &vol)) { const std::string e = scn_last_error(); scn_sens_close(s); return scn::fail(SCN_ERR_CUDA, "%s", e.c_str()); }
+    if (int r = scn_tsdf_create(&p, job.device, &vol)) return scn::fail(r, "%s: %s", job.sens_path.c_str(), scn_last_error());
     vs->vol = vol; vs->p = p;
   }
   const size_t px = (size_t)in.depth_width * in.depth_height;
@@ -171,128 +173,108 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
   rep.gpu_decode = gpu_decode ? 1 : 0;
   const double t0 = now_s();
   rep.setup_s = t0 - t_begin;
-  int rc = 0; std::string err;
-  auto fail_here = [&](const char* what) { if (!rc) { rc = 1; err = what && *what ? what : scn_last_error(); } };
+  FirstFailure fail;
+  double tt0 = 0;                                  // GPU decode: start of the teardown, which ends when the decode buffers are released
   if (gpu_decode) {
     const char* ce = getenv("SCN_FUSE_CHUNK");
     const uint32_t CH = (uint32_t)std::max(16, std::min(4096, ce ? atoi(ce) : 1024));   // frames per decode chunk: enough streams in flight for the one-warp-per-frame decoders
     const uint64_t n_chunks = (in.n_frames + CH - 1) / CH;
-    uint16_t* d_depth[2] = {nullptr, nullptr}; uint8_t* d_rgb[2] = {nullptr, nullptr}; int32_t* d_lut = nullptr;
-    void* st_d = nullptr; void* st_c = nullptr;
+    uint16_t* d_depth[2] = {nullptr, nullptr}; uint8_t* d_rgb[2] = {nullptr, nullptr};
+    scn::DevicePtr<int32_t> d_lut; scn::HandleStreamPtr st_d, st_c; scn::PinnedPtr<uint8_t> h_rgb;
     scn::StagePool<FrameBufs>::Lease fb(frame_pool());
     for (int b = 0; b < 2; ++b) {
       d_depth[b] = (uint16_t*)fb->take(b, (size_t)CH * px * 2);
       if (use_color) d_rgb[b] = (uint8_t*)fb->take(2 + b, (size_t)CH * px * 3);
-      if (!d_depth[b] || (use_color && !d_rgb[b])) fail_here(nullptr);
+      if (!d_depth[b] || (use_color && !d_rgb[b])) fail.set(SCN_ERR_CUDA);
     }
-    if (use_color && !rc) { d_lut = (int32_t*)scn_device_alloc(px * 4); if (!d_lut || scn_memcpy_h2d(d_lut, lut.data(), px * 4, nullptr)) fail_here(nullptr); }
-    if (!rc && (scn_stream_create(&st_d) || scn_stream_create(&st_c))) fail_here(nullptr);
+    if (use_color && !fail) {
+      d_lut.reset((int32_t*)scn_device_alloc(px * 4));
+      if (int r = d_lut ? scn_memcpy_h2d(d_lut.get(), lut.data(), px * 4, nullptr) : SCN_ERR_CUDA) fail.set(r);
+    }
+    if (!fail) { int r = scn::create(st_d); if (!r) r = scn::create(st_c); if (r) fail.set(r); }
     rep.buffers_s = now_s() - t0;
-    // per chunk: the frames with a valid pose, compacted (a frame without a pose is never decoded: sensorData.h:382)
-    struct ChunkPlan { std::vector<uint64_t> frames; std::vector<float> poses; };
     std::mutex m; std::condition_variable cv;
     std::vector<int> depth_done(n_chunks, 0), color_done(n_chunks, 0);            // 1 = ready, -1 = failed
-    std::vector<ChunkPlan> plan(n_chunks);
+    std::vector<scn::PosedFrames> plan(n_chunks);
     uint64_t consumed = 0;                                                          // chunks whose buffers are free again
-    std::string dec_err; bool stop = false;
-    for (uint64_t c = 0; c < n_chunks; ++c) {
+    bool stop = false;
+    for (uint64_t c = 0; c < n_chunks && !fail; ++c) {
       const uint64_t f0 = c * CH, f1 = std::min<uint64_t>(in.n_frames, f0 + CH);
-      for (uint64_t f = f0; f < f1; ++f) {
-        float T[16]; scn_sens_frame_meta(s, f, T, nullptr, nullptr, nullptr, nullptr);
-        if (T[0] == -INFINITY) { ++rep.frames_skipped_pose; continue; }
-        plan[c].frames.push_back(f); plan[c].poses.insert(plan[c].poses.end(), T, T + 16);
-      }
+      if (int r = scn::posed_frames(s, f0, f1, plan[c])) fail.set(r);
+      else rep.frames_skipped_pose += (f1 - f0) - plan[c].frames.size();
     }
     std::unique_ptr<Pool> color_pool;
     if (use_color && in.color_compression != 2) color_pool.reset(new Pool(std::max(1u, std::min(32u, std::thread::hardware_concurrency())) - 1));
-    uint8_t* h_rgb = nullptr;
     auto decoder = [&](bool is_color) {
       scn_set_device(job.device);
       std::vector<const uint8_t*> src; std::vector<uint64_t> len;
       for (uint64_t c = 0; c < n_chunks; ++c) {
         { std::unique_lock<std::mutex> l(m); cv.wait(l, [&]() { return stop || c < consumed + 2; }); if (stop) return; }
-        const ChunkPlan& pl = plan[c];
+        const scn::PosedFrames& pl = plan[c];
         const uint32_t n = (uint32_t)pl.frames.size();
-        int r = 0; std::string e;
+        int r = 0;
         if (n) {
-          src.resize(n); len.resize(n);
-          for (uint32_t i = 0; i < n; ++i) {
-            const uint8_t* cp = nullptr; const uint8_t* dp = nullptr; uint64_t cb = 0, db = 0;
-            scn_sens_frame_payload(s, pl.frames[i], &cp, &dp);
-            scn_sens_frame_meta(s, pl.frames[i], nullptr, nullptr, nullptr, &cb, &db);
-            src[i] = is_color ? cp : dp; len[i] = is_color ? cb : db;
-          }
           const double td0 = now_s();
-          if (is_color && in.color_compression != 2) {
+          if (!is_color) {
+            r = scn::sens_depth_to_device(s, pl.frames.data(), n, d_depth[c & 1], st_d.get());
+            double ps = 0, km = 0; scn_inflate_last_timings(&ps, &km, nullptr, nullptr);
+            if (!r) { std::lock_guard<std::mutex> l(m); rep.depth_decode_s += now_s() - td0; rep.depth_pack_s += ps; rep.depth_kernel_s += km * 1e-3; }
+          } else if (in.color_compression != 2) {
             // raw / PNG colour: host pool into a pinned chunk (registered to depth on the way), one upload
-            if (!h_rgb) h_rgb = (uint8_t*)scn_host_alloc((size_t)CH * px * 3);
+            if (!h_rgb) h_rgb.reset((uint8_t*)scn_host_alloc((size_t)CH * px * 3));
             if (!h_rgb) r = SCN_ERR_CUDA;
-            std::atomic<uint32_t> nx{0}; std::atomic<int> prc{0}; std::mutex pem; std::string perr;
-            auto work = [&]() {
+            std::atomic<uint32_t> nx{0};
+            if (!r) color_pool->run([&]() {
               static thread_local std::vector<uint8_t> col;
               col.resize((size_t)in.color_width * in.color_height * 3);
-              for (;;) {
-                const uint32_t i = nx.fetch_add(1);
-                if (i >= n || prc.load() || r) break;
-                const int q = scn_sens_frame_color_rgb8(s, pl.frames[i], col.data());
-                if (q) { std::lock_guard<std::mutex> l(pem); if (!prc.load()) { perr = scn_last_error(); prc.store(q); } break; }
-                uint8_t* o = h_rgb + (size_t)i * px * 3;
-                for (size_t pp = 0; pp < px; ++pp) { const int32_t qq = lut[pp]; if (qq >= 0) { o[3 * pp] = col[3 * (size_t)qq]; o[3 * pp + 1] = col[3 * (size_t)qq + 1]; o[3 * pp + 2] = col[3 * (size_t)qq + 2]; } else o[3 * pp] = o[3 * pp + 1] = o[3 * pp + 2] = 0; }
-              }
-            };
-            if (!r) { color_pool->run(work); r = prc.load(); if (r) scn::fail(r, "%s", perr.c_str()); }
-            if (!r) r = scn_memcpy_h2d(d_rgb[c & 1], h_rgb, (size_t)n * px * 3, st_c);
+              for (uint32_t i; (i = nx.fetch_add(1)) < n && !fail;)
+                if (int q = scn::sens_color_to_depth(s, pl.frames[i], lut.data(), px, col.data(), h_rgb.get() + (size_t)i * px * 3)) fail.set(q);
+            });
+            if (!r) r = fail.rc.load();                                           // the scene failed (here or elsewhere): no upload
+            if (!r) r = scn_memcpy_h2d(d_rgb[c & 1], h_rgb.get(), (size_t)n * px * 3, st_c.get());
             if (!r) { std::lock_guard<std::mutex> l(m); rep.color_decode_s += now_s() - td0; }
-          } else if (is_color) {
+          } else {
+            src.resize(n); len.resize(n);
+            for (uint32_t i = 0; i < n && !r; ++i)
+              if (!(r = scn_sens_frame_payload(s, pl.frames[i], &src[i], nullptr))) r = scn_sens_frame_meta(s, pl.frames[i], nullptr, nullptr, nullptr, &len[i], nullptr);
             uint32_t k = 0;
-            r = scn_jpeg_decode_batch_device(src.data(), len.data(), n, in.color_width, in.color_height, d_lut, (uint32_t)px, d_rgb[c & 1], st_c, &k);
+            if (!r) r = scn_jpeg_decode_batch_device(src.data(), len.data(), n, in.color_width, in.color_height, d_lut.get(), (uint32_t)px, d_rgb[c & 1], st_c.get(), &k);
             double hs = 0, em = 0, cm = 0; scn_jpeg_last_timings(&hs, &em, &cm);
             if (!r) { std::lock_guard<std::mutex> l(m); rep.color_frames_on_device += k; rep.color_decode_s += now_s() - td0;
                       rep.color_host_s += hs; rep.color_entropy_s += em * 1e-3; rep.color_convert_s += cm * 1e-3; }
-          } else if (in.depth_compression == 1) {
-            r = scn_inflate_batch_device(src.data(), len.data(), n, (uint64_t)px * 2, d_depth[c & 1], st_d);
-            double ps = 0, km = 0; scn_inflate_last_timings(&ps, &km, nullptr, nullptr);
-            if (!r) { std::lock_guard<std::mutex> l(m); rep.depth_decode_s += now_s() - td0; rep.depth_pack_s += ps; rep.depth_kernel_s += km * 1e-3; }
-          } else {
-            for (uint32_t i = 0; i < n && !r; ++i) {
-              if (len[i] < px * 2) { r = scn::fail(SCN_ERR_FORMAT, "frame %llu: invalid data", (unsigned long long)pl.frames[i]); break; }
-              r = scn_memcpy_h2d(d_depth[c & 1] + (size_t)i * px, src[i], px * 2, st_d);
-            }
           }
-          if (r) e = scn_last_error();
         }
-        { std::lock_guard<std::mutex> l(m); (is_color ? color_done : depth_done)[c] = r ? -1 : 1; if (r && dec_err.empty()) dec_err = e; }
+        if (r) fail.set(r);
+        { std::lock_guard<std::mutex> l(m); (is_color ? color_done : depth_done)[c] = r ? -1 : 1; }
         cv.notify_all();
         if (r) return;
       }
     };
     std::thread th_d, th_c;
-    if (!rc) { th_d = std::thread(decoder, false); if (use_color) th_c = std::thread(decoder, true); }
-    for (uint64_t c = 0; c < n_chunks && !rc; ++c) {
+    if (!fail) { th_d = std::thread(decoder, false); if (use_color) th_c = std::thread(decoder, true); }
+    for (uint64_t c = 0; c < n_chunks && !fail; ++c) {
       const double tw0 = now_s();
       {
         std::unique_lock<std::mutex> l(m);
         cv.wait(l, [&]() { return depth_done[c] != 0 && (!use_color || color_done[c] != 0); });
-        if (depth_done[c] < 0 || (use_color && color_done[c] < 0)) { fail_here(dec_err.c_str()); break; }
+        if (depth_done[c] < 0 || (use_color && color_done[c] < 0)) break;
       }
       rep.decode_wait_s += now_s() - tw0;
-      const ChunkPlan& pl = plan[c];
+      const scn::PosedFrames& pl = plan[c];
       if (!pl.frames.empty()) {
         const double ti0 = now_s();
-        if (scn_tsdf_integrate_device(vol, (uint32_t)pl.frames.size(), d_depth[c & 1], use_color ? d_rgb[c & 1] : nullptr, pl.poses.data(), in.depth_intrinsic)) { fail_here(nullptr); break; }
-        if (scn_tsdf_sync(vol)) { fail_here(nullptr); break; }                          // the buffers of this chunk may be overwritten now
+        if (int r = scn_tsdf_integrate_device(vol, (uint32_t)pl.frames.size(), d_depth[c & 1], use_color ? d_rgb[c & 1] : nullptr, pl.poses.data(), in.depth_intrinsic)) { fail.set(r); break; }
+        if (int r = scn_tsdf_sync(vol)) { fail.set(r); break; }                         // the buffers of this chunk may be overwritten now
         rep.integrate_s += now_s() - ti0;
       }
       { std::lock_guard<std::mutex> l(m); consumed = c + 1; }
       cv.notify_all();
     }
-    const double tt0 = now_s();
+    tt0 = now_s();
     { std::lock_guard<std::mutex> l(m); stop = true; }
     cv.notify_all();
     if (th_d.joinable()) th_d.join();
     if (th_c.joinable()) th_c.join();
-    scn_device_free(d_lut); scn_stream_destroy(st_d); scn_stream_destroy(st_c); scn_host_free(h_rgb);
-    rep.teardown_s = now_s() - tt0;
   } else {
     // host decode is the bottleneck of this mode (one frame = ~2 ms inflate + ~1-3 ms JPEG on one core): up to 64 cores,
     // chunks of two frames per worker
@@ -300,24 +282,26 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
     const uint32_t CH = std::max(32u, 2 * threads);
     Pool pool(threads - 1);
     Chunk ch[2];
-    for (Chunk& c : ch) { c.depth = (uint16_t*)scn_host_alloc(CH * px * 2); c.rgb = use_color ? (uint8_t*)scn_host_alloc(CH * px * 3) : nullptr;
-      if (!c.depth || (use_color && !c.rgb)) fail_here(nullptr); }
+    for (Chunk& c : ch) {
+      c.depth.reset((uint16_t*)scn_host_alloc(CH * px * 2));
+      if (use_color) c.rgb.reset((uint8_t*)scn_host_alloc(CH * px * 3));
+      if (!c.depth || (use_color && !c.rgb)) fail.set(SCN_ERR_CUDA);
+    }
     uint64_t f = 0; int cur = 0;
-    if (!rc && in.n_frames) decode_chunk(s, in, lut, use_color, 0, (uint32_t)std::min<uint64_t>(CH, in.n_frames), ch[0], pool);
-    while (f < in.n_frames && !rc) {
+    if (!fail && in.n_frames) decode_chunk(s, in, lut, use_color, 0, (uint32_t)std::min<uint64_t>(CH, in.n_frames), ch[0], pool, fail);
+    while (f < in.n_frames && !fail) {
       Chunk& c = ch[cur];
-      if (c.rc) { fail_here(c.err.c_str()); break; }
       // the GPU consumes chunk `cur` asynchronously while the host decodes the next one into the other buffer
-      if (scn_tsdf_integrate_batch(vol, c.n, c.depth, c.rgb, c.poses.data(), in.depth_intrinsic)) { fail_here(nullptr); break; }
+      if (int r = scn_tsdf_integrate_batch(vol, c.n, c.depth.get(), c.rgb.get(), c.poses.data(), in.depth_intrinsic)) { fail.set(r); break; }
       f += c.n;
-      if (f < in.n_frames) decode_chunk(s, in, lut, use_color, f, (uint32_t)std::min<uint64_t>(CH, in.n_frames - f), ch[cur ^ 1], pool);
-      if (scn_tsdf_sync(vol)) { fail_here(nullptr); break; }      // chunk `cur` may be overwritten next round
+      if (f < in.n_frames) decode_chunk(s, in, lut, use_color, f, (uint32_t)std::min<uint64_t>(CH, in.n_frames - f), ch[cur ^ 1], pool, fail);
+      if (int r = scn_tsdf_sync(vol)) { fail.set(r); break; }      // chunk `cur` may be overwritten next round
       cur ^= 1;
     }
-    for (Chunk& c : ch) { scn_host_free(c.depth); scn_host_free(c.rgb); }
   }
+  if (gpu_decode) rep.teardown_s = now_s() - tt0;
   rep.fuse_s = now_s() - t0;
-  if (!rc) {
+  if (!fail) {
     scn_tsdf_stats_t st; scn_tsdf_stats(vol, &st);
     rep.frames_integrated = st.frames_integrated; rep.frames_skipped = st.frames_skipped + rep.frames_skipped_pose;
     rep.blocks_allocated = st.blocks_allocated; rep.voxels_updated = st.voxels_updated;
@@ -330,20 +314,20 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
     if (!job.out_path.empty()) {
       const double tm0 = now_s();
       float* xyz = nullptr; uint8_t* rgb = nullptr; uint32_t* tri = nullptr; uint64_t nV = 0, nF = 0;
-      if (scn_tsdf_extract_mesh(vol, &xyz, &rgb, &tri, &nV, &nF)) fail_here(nullptr);
+      if (int r = scn_tsdf_extract_mesh(vol, &xyz, &rgb, &tri, &nV, &nF)) fail.set(r);
+      const scn::MallocPtr<float> own_xyz(xyz); const scn::MallocPtr<uint8_t> own_rgb(rgb); const scn::MallocPtr<uint32_t> own_tri(tri);
       rep.mc_s = now_s() - tm0;
-      if (!rc && scn_mesh_save_ply(job.out_path.c_str(), xyz, use_color ? rgb : nullptr, nV, tri, nF)) fail_here(nullptr);
+      if (!fail) { if (int r = scn_mesh_save_ply(job.out_path.c_str(), xyz, use_color ? rgb : nullptr, nV, tri, nF)) fail.set(r); }
       rep.ply_s = now_s() - tm0 - rep.mc_s;
       rep.mesh_vertices = nV; rep.mesh_faces = nF;
-      if (!rc && job.verbose) printf("mesh written to %s with %llu vertices, %llu faces\n", job.out_path.c_str(), (unsigned long long)nV, (unsigned long long)nF);
-      scn_free(xyz); scn_free(rgb); scn_free(tri);
+      if (!fail && job.verbose) printf("mesh written to %s with %llu vertices, %llu faces\n", job.out_path.c_str(), (unsigned long long)nV, (unsigned long long)nF);
     }
   }
-  if (rc) vs->release();                                       // do not hand a volume of unknown state to the next scene
-  scn_sens_close(s);
+  if (fail) vs->release();                                     // do not hand a volume of unknown state to the next scene
+  sens.reset();                                                // total_s includes unmapping the file
   rep.total_s = now_s() - t_begin;
   if (rep_out) *rep_out = rep;
-  return rc ? scn::fail(SCN_ERR_FORMAT, "%s: %s", job.sens_path.c_str(), err.c_str()) : SCN_OK;
+  return fail ? scn::fail(fail.rc.load(), "%s: %s", job.sens_path.c_str(), fail.err.c_str()) : SCN_OK;
 }
 
 std::string default_out(const std::string& sens_path) { return sens_path.substr(0, sens_path.size() - 5) + "_vh.ply"; }

@@ -610,27 +610,32 @@ int scn_inflate_last_timings(double* pack_s, double* kernel_ms, int* ring_window
 int scn_sens_decode_depth_device(const scn_sens* s, uint64_t first, uint32_t n, uint16_t* d_depth_out, void* stream) {
   if (!s || (!d_depth_out && n)) return scn::fail(SCN_ERR_ARG, "null argument");
   scn_sens_info_t info;
-  if (scn_sens_info(s, &info)) return SCN_ERR_ARG;
+  if (int rc = scn_sens_info(s, &info)) return rc;
   if (first + n > info.n_frames) return scn::fail(SCN_ERR_ARG, "out of bounds");
-  const uint64_t fb = (uint64_t)info.depth_width * info.depth_height * 2;
-  if (info.depth_compression == 2) return scn::fail(SCN_ERR_UNSUPPORTED, "need UPLINK_COMPRESSION");
-  if (info.depth_compression != 0 && info.depth_compression != 1) return scn::fail(SCN_ERR_FORMAT, "invalid type");
-  std::vector<const uint8_t*> src(n); std::vector<uint64_t> len(n);
-  for (uint32_t i = 0; i < n; ++i) {
-    const uint8_t* c = nullptr; const uint8_t* d = nullptr; uint64_t db = 0;
-    if (scn_sens_frame_payload(s, first + i, &c, &d) || scn_sens_frame_meta(s, first + i, nullptr, nullptr, nullptr, nullptr, &db)) return SCN_ERR_ARG;
-    src[i] = d; len[i] = db;
-  }
-  if (info.depth_compression == 0) {
-    cudaStream_t st = (cudaStream_t)stream;
-    for (uint32_t i = 0; i < n; ++i) {
-      if (len[i] < fb) return scn::fail(SCN_ERR_FORMAT, "invalid data");
-      SCN_CUDA_TRY(cudaMemcpyAsync((uint8_t*)d_depth_out + (size_t)i * fb, src[i], fb, cudaMemcpyHostToDevice, st));
-    }
-    SCN_CUDA_TRY(cudaStreamSynchronize(st));
-    return SCN_OK;
-  }
-  return scn_inflate_batch_device(src.data(), len.data(), n, fb, d_depth_out, stream);
+  std::vector<uint64_t> frames(n);
+  for (uint32_t i = 0; i < n; ++i) frames[i] = first + i;
+  return scn::sens_depth_to_device(s, frames.data(), n, d_depth_out, stream);
 }
 
 }  // extern "C"
+
+int scn::sens_depth_to_device(const scn_sens* s, const uint64_t* frames, uint32_t n, uint16_t* d_out, void* stream) {
+  scn_sens_info_t info;
+  if (int rc = scn_sens_info(s, &info)) return rc;
+  if (info.depth_compression == 2) return scn::fail(SCN_ERR_UNSUPPORTED, "need UPLINK_COMPRESSION");
+  if (info.depth_compression != 0 && info.depth_compression != 1) return scn::fail(SCN_ERR_FORMAT, "invalid type");
+  const uint64_t fb = (uint64_t)info.depth_width * info.depth_height * 2;
+  std::vector<const uint8_t*> src(n); std::vector<uint64_t> len(n);
+  for (uint32_t i = 0; i < n; ++i) {
+    if (int rc = scn_sens_frame_payload(s, frames[i], nullptr, &src[i])) return rc;
+    if (int rc = scn_sens_frame_meta(s, frames[i], nullptr, nullptr, nullptr, nullptr, &len[i])) return rc;
+    if (info.depth_compression == 0 && len[i] < fb)
+      return scn::fail(SCN_ERR_FORMAT, "frame %llu: raw depth payload of %llu bytes, need %llu", (unsigned long long)frames[i],
+                       (unsigned long long)len[i], (unsigned long long)fb);
+  }
+  if (info.depth_compression == 1) return scn_inflate_batch_device(src.data(), len.data(), n, fb, d_out, stream);
+  cudaStream_t st = (cudaStream_t)stream;
+  for (uint32_t i = 0; i < n; ++i) SCN_CUDA_TRY(cudaMemcpyAsync((uint8_t*)d_out + (size_t)i * fb, src[i], fb, cudaMemcpyHostToDevice, st));
+  SCN_CUDA_TRY(cudaStreamSynchronize(st));
+  return SCN_OK;
+}

@@ -680,13 +680,10 @@ int scn_sens_decode_color_device(const scn_sens* s, uint64_t first, uint32_t n, 
   if (d_lut) { lut.resize(out_px); SCN_CUDA_TRY(cudaMemcpyAsync(lut.data(), d_lut, (size_t)out_px * 4, cudaMemcpyDeviceToHost, st)); SCN_CUDA_TRY(cudaStreamSynchronize(st)); }
   std::vector<uint8_t> full((size_t)info.color_width * info.color_height * 3), res((size_t)(d_lut ? out_px : 0) * 3);
   for (uint32_t i = 0; i < n; ++i) {
-    const int rc = scn_sens_frame_color_rgb8(s, first + i, full.data());
+    const int rc = d_lut ? scn::sens_color_to_depth(s, first + i, lut.data(), out_px, full.data(), res.data())
+                         : scn_sens_frame_color_rgb8(s, first + i, full.data());
     if (rc) return rc;
-    const uint8_t* h = full.data();
-    if (d_lut) {
-      for (uint32_t p = 0; p < out_px; ++p) { const int32_t q = lut[p]; if (q >= 0) { res[3 * (size_t)p] = full[3 * (size_t)q]; res[3 * (size_t)p + 1] = full[3 * (size_t)q + 1]; res[3 * (size_t)p + 2] = full[3 * (size_t)q + 2]; } else res[3 * (size_t)p] = res[3 * (size_t)p + 1] = res[3 * (size_t)p + 2] = 0; }
-      h = res.data();
-    }
+    const uint8_t* h = d_lut ? res.data() : full.data();
     SCN_CUDA_TRY(cudaMemcpyAsync((uint8_t*)d_out + (size_t)i * out_px * 3, h, (size_t)out_px * 3, cudaMemcpyHostToDevice, st));
     SCN_CUDA_TRY(cudaStreamSynchronize(st));
   }

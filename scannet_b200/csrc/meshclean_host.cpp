@@ -96,6 +96,21 @@ size_t tag_end(const std::string& xml, size_t pos) {
   return std::string::npos;
 }
 
+// the lines of the clean filters that ran: their counters, and the size of the mesh they left
+void print_clean(const scn_mesh_clean_params& p, const scn_mesh_clean_report_t& r, uint64_t oV, uint64_t oF) {
+  if (!(p.flags & SCN_CLEAN_SKIP_MERGE))
+    printf("Merge Close Vertices (%g): %llu vertices merged, %llu degenerate faces removed (%.2f ms)\n", (double)p.merge_threshold,
+           (unsigned long long)r.vertices_merged, (unsigned long long)r.degenerate_faces, r.merge_ms);
+  if (!(p.flags & SCN_CLEAN_SKIP_DEDUP))
+    printf("Remove Duplicate Faces: %llu faces removed (%.2f ms)\n", (unsigned long long)r.duplicate_faces, r.dedup_ms);
+  if (!(p.flags & SCN_CLEAN_SKIP_PIECES)) {
+    printf("Remove Isolated pieces (min %u faces, %u vertices): %llu of %llu pieces removed, %llu faces (%.2f ms)\n", p.min_piece_faces,
+           p.min_piece_vertices, (unsigned long long)r.pieces_removed, (unsigned long long)r.pieces_total,
+           (unsigned long long)r.faces_in_removed_pieces, r.pieces_ms);
+    printf("Remove Unreferenced Vertex: %llu vertices, %llu faces remain\n", (unsigned long long)oV, (unsigned long long)oF);
+  }
+}
+
 bool read_file(const char* path, std::string& xml) {
   std::ifstream in(path, std::ios::binary);
   if (!in) return false;
@@ -138,30 +153,19 @@ int scn_meshclean_main(int argc, const char** argv) {
   scn_mesh_clean_params p;
   scn_mesh_clean_default_params(&p);
   if (script && scn_mesh_clean_params_from_mlx(script, &p)) { warm.join(); fprintf(stderr, "%s\n", scn_last_error()); return 1; }
-  float* xyz = nullptr; uint8_t* rgb = nullptr; uint32_t* tri = nullptr; uint64_t nV = 0, nF = 0;
-  const int lrc = scn_mesh_load_rgb(in, &xyz, &rgb, &nV, &tri, &nF);
+  float* x = nullptr; uint8_t* c = nullptr; uint32_t* t = nullptr; uint64_t nV = 0, nF = 0;
+  const int lrc = scn_mesh_load_rgb(in, &x, &c, &nV, &t, &nF);
+  const scn::MallocPtr<float> xyz(x); const scn::MallocPtr<uint8_t> rgb(c); const scn::MallocPtr<uint32_t> tri(t);
   warm.join();
   if (lrc) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
   printf("Loaded %s: %llu vertices, %llu faces%s\n", in, (unsigned long long)nV, (unsigned long long)nF, rgb ? ", vertex colour" : "");
-  float* oxyz = nullptr; uint8_t* orgb = nullptr; uint32_t* otri = nullptr; uint64_t oV = 0, oF = 0;
+  float* ox = nullptr; uint8_t* oc = nullptr; uint32_t* ot = nullptr; uint64_t oV = 0, oF = 0;
   scn_mesh_clean_report_t r;
-  const int crc = scn_mesh_clean(xyz, vc ? rgb : nullptr, nV, tri, nF, &p, &oxyz, &orgb, &otri, &oV, &oF, &r);
-  scn_free(xyz); scn_free(rgb); scn_free(tri);
+  const int crc = scn_mesh_clean(xyz.get(), vc ? rgb.get() : nullptr, nV, tri.get(), nF, &p, &ox, &oc, &ot, &oV, &oF, &r);
+  const scn::MallocPtr<float> oxyz(ox); const scn::MallocPtr<uint8_t> orgb(oc); const scn::MallocPtr<uint32_t> otri(ot);
   if (crc) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
-  if (!(p.flags & SCN_CLEAN_SKIP_MERGE))
-    printf("Merge Close Vertices (%g): %llu vertices merged, %llu degenerate faces removed (%.2f ms)\n", (double)p.merge_threshold,
-           (unsigned long long)r.vertices_merged, (unsigned long long)r.degenerate_faces, r.merge_ms);
-  if (!(p.flags & SCN_CLEAN_SKIP_DEDUP))
-    printf("Remove Duplicate Faces: %llu faces removed (%.2f ms)\n", (unsigned long long)r.duplicate_faces, r.dedup_ms);
-  if (!(p.flags & SCN_CLEAN_SKIP_PIECES)) {
-    printf("Remove Isolated pieces (min %u faces, %u vertices): %llu of %llu pieces removed, %llu faces (%.2f ms)\n", p.min_piece_faces,
-           p.min_piece_vertices, (unsigned long long)r.pieces_removed, (unsigned long long)r.pieces_total,
-           (unsigned long long)r.faces_in_removed_pieces, r.pieces_ms);
-    printf("Remove Unreferenced Vertex: %llu vertices, %llu faces remain\n", (unsigned long long)oV, (unsigned long long)oF);
-  }
-  const int src = scn_mesh_save_ply(out, oxyz, orgb, oV, otri, oF);
-  scn_free(oxyz); scn_free(orgb); scn_free(otri);
-  if (src) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
+  print_clean(p, r, oV, oF);
+  if (scn_mesh_save_ply(out, oxyz.get(), orgb.get(), oV, otri.get(), oF)) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
   printf("Saved %s: %llu vertices, %llu faces\n", out, (unsigned long long)oV, (unsigned long long)oF);
   return 0;
 }
@@ -247,35 +251,24 @@ int scn_meshsimplify_main(int argc, const char** argv) {
   scn_mesh_clean_params c;
   scn_mesh_simplify_default_params(&p, &c);
   if (script && scn_mesh_simplify_params_from_mlx(script, &p, &c)) { warm.join(); fprintf(stderr, "%s\n", scn_last_error()); return 1; }
-  float* xyz = nullptr; uint8_t* rgb = nullptr; uint32_t* tri = nullptr; uint64_t nV = 0, nF = 0;
-  const int lrc = scn_mesh_load_rgb(in, &xyz, &rgb, &nV, &tri, &nF);
+  float* x = nullptr; uint8_t* cl = nullptr; uint32_t* t = nullptr; uint64_t nV = 0, nF = 0;
+  const int lrc = scn_mesh_load_rgb(in, &x, &cl, &nV, &t, &nF);
+  const scn::MallocPtr<float> xyz(x); const scn::MallocPtr<uint8_t> rgb(cl); const scn::MallocPtr<uint32_t> tri(t);
   warm.join();
   if (lrc) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
   printf("Loaded %s: %llu vertices, %llu faces%s\n", in, (unsigned long long)nV, (unsigned long long)nF, rgb ? ", vertex colour" : "");
-  float* oxyz = nullptr; uint8_t* orgb = nullptr; uint32_t* otri = nullptr; uint64_t oV = 0, oF = 0;
+  float* ox = nullptr; uint8_t* oc = nullptr; uint32_t* ot = nullptr; uint64_t oV = 0, oF = 0;
   scn_mesh_simplify_report_t r;
-  const int crc = scn_mesh_simplify(xyz, vc ? rgb : nullptr, nV, tri, nF, &p, &c, &oxyz, &orgb, &otri, &oV, &oF, &r);
-  scn_free(xyz); scn_free(rgb); scn_free(tri);
+  const int crc = scn_mesh_simplify(xyz.get(), vc ? rgb.get() : nullptr, nV, tri.get(), nF, &p, &c, &ox, &oc, &ot, &oV, &oF, &r);
+  const scn::MallocPtr<float> oxyz(ox); const scn::MallocPtr<uint8_t> orgb(oc); const scn::MallocPtr<uint32_t> otri(ot);
   if (crc) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
   printf("Quadric Edge Collapse Decimation (target %llu faces, quality threshold %g): %llu collapses in %llu rounds removed %llu faces; "
          "AutoClean removed %llu duplicate faces, %llu vertices, %llu faces remain (%.2f ms)\n", (unsigned long long)r.target_faces,
          p.quality_thr, (unsigned long long)r.collapses, (unsigned long long)r.rounds, (unsigned long long)r.faces_collapsed,
          (unsigned long long)r.autoclean_duplicate_faces, (unsigned long long)r.clean.vertices_in, (unsigned long long)r.clean.faces_in,
          r.quadrics_ms + r.rounds_ms + r.autoclean_ms);
-  if (!(c.flags & SCN_CLEAN_SKIP_MERGE))
-    printf("Merge Close Vertices (%g): %llu vertices merged, %llu degenerate faces removed (%.2f ms)\n", (double)c.merge_threshold,
-           (unsigned long long)r.clean.vertices_merged, (unsigned long long)r.clean.degenerate_faces, r.clean.merge_ms);
-  if (!(c.flags & SCN_CLEAN_SKIP_DEDUP))
-    printf("Remove Duplicate Faces: %llu faces removed (%.2f ms)\n", (unsigned long long)r.clean.duplicate_faces, r.clean.dedup_ms);
-  if (!(c.flags & SCN_CLEAN_SKIP_PIECES)) {
-    printf("Remove Isolated pieces (min %u faces, %u vertices): %llu of %llu pieces removed, %llu faces (%.2f ms)\n", c.min_piece_faces,
-           c.min_piece_vertices, (unsigned long long)r.clean.pieces_removed, (unsigned long long)r.clean.pieces_total,
-           (unsigned long long)r.clean.faces_in_removed_pieces, r.clean.pieces_ms);
-    printf("Remove Unreferenced Vertex: %llu vertices, %llu faces remain\n", (unsigned long long)oV, (unsigned long long)oF);
-  }
-  const int src = scn_mesh_save_ply(out, oxyz, orgb, oV, otri, oF);
-  scn_free(oxyz); scn_free(orgb); scn_free(otri);
-  if (src) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
+  print_clean(c, r.clean, oV, oF);
+  if (scn_mesh_save_ply(out, oxyz.get(), orgb.get(), oV, otri.get(), oF)) { fprintf(stderr, "%s\n", scn_last_error()); return 1; }
   printf("Saved %s: %llu vertices, %llu faces\n", out, (unsigned long long)oV, (unsigned long long)oF);
   return 0;
 }

@@ -1,12 +1,15 @@
 // Shared host-side helpers for libscannet_b200.so: thread-local error text, CUDA status checks, scoped owners of CUDA
-// resources.
+// resources and of the C-ABI handles, and the .sens frame helpers the scene drivers share.
 #pragma once
+#include <chrono>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <string>
+#include <vector>
 
 #include "../../include/scannet_b200.h"
 
@@ -15,12 +18,35 @@ namespace scn {
 std::string& last_error_ref();
 int fail(int code, const char* fmt, ...);
 
+inline double now_s() { return std::chrono::duration<double>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
+
+// Host-side owners: std::unique_ptr with the matching release call.  A malloc'd result is handed to the caller with release();
+// the arrays the library hands out are released with MallocPtr, as scn_free is free.
+template <auto fn> struct Release { template <class P> void operator()(P p) const { fn(p); } };
+template <class T> using MallocPtr = std::unique_ptr<T[], Release<free>>;
+template <class T> using PinnedPtr = std::unique_ptr<T[], Release<scn_host_free>>;
+template <class T> using DevicePtr = std::unique_ptr<T[], Release<scn_device_free>>;
+using SensPtr = std::unique_ptr<scn_sens, Release<scn_sens_close>>;
+using FreespacePtr = std::unique_ptr<scn_freespace, Release<scn_freespace_destroy>>;
+using HandleStreamPtr = std::unique_ptr<void, Release<scn_stream_destroy>>;        // a scn_stream_create stream
+inline int create(HandleStreamPtr& st) { void* x = nullptr; const int rc = scn_stream_create(&x); st.reset(x); return rc; }
+
+// .sens helpers of the scene drivers (sens.cpp, inflate.cu)
+struct PosedFrames { std::vector<uint64_t> frames; std::vector<float> poses; };     // poses: 16 floats per frame
+// The frames of [f0, f1) that have a pose, with their poses (a frame without one is never decoded: sensorData.h:382).
+int posed_frames(const scn_sens* s, uint64_t f0, uint64_t f1, PosedFrames& out);
+// Decodes the colour of `frame` into `scratch` (color_width x color_height RGB8) and registers it to the depth image:
+// out[p] = scratch[lut[p]], black where lut[p] < 0, for the n_px depth pixels.
+int sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, size_t n_px, uint8_t* scratch, uint8_t* out);
+// The depth of frames[0..n) into device memory, frame after frame (u16, row-major): zlib streams through the GPU inflate, raw
+// frames uploaded.  Returns when the frames are on the device.
+int sens_depth_to_device(const scn_sens* s, const uint64_t* frames, uint32_t n, uint16_t* d_out, void* stream);
+
 }  // namespace scn
 
 #ifdef __CUDACC__
 #include <cuda_runtime.h>
 
-#include <memory>
 #include <utility>
 
 #define SCN_CUDA_TRY(expr)                                                                   \
@@ -48,10 +74,6 @@ struct DBuf {
 };
 #define SCN_ALLOC(buf, bytes) do { if (!(buf).alloc(bytes)) return scn::fail(SCN_ERR_CUDA, "cudaMalloc(%zu) failed (%s:%d)", (size_t)(bytes), __FILE__, __LINE__); } while (0)
 
-// Host-side owners: std::unique_ptr with the matching release call.  A malloc'd result is handed to the caller with release().
-template <auto fn> struct Release { template <class P> void operator()(P p) const { fn(p); } };
-template <class T> using PinnedPtr = std::unique_ptr<T[], Release<cudaFreeHost>>;
-template <class T> using MallocPtr = std::unique_ptr<T[], Release<free>>;
 using EventPtr = std::unique_ptr<CUevent_st, Release<cudaEventDestroy>>;
 using StreamPtr = std::unique_ptr<CUstream_st, Release<cudaStreamDestroy>>;
 

@@ -783,3 +783,24 @@ int scn_sens_main(int argc, const char** argv) {
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------ frame helpers of the scene drivers
+int scn::posed_frames(const scn_sens* s, uint64_t f0, uint64_t f1, PosedFrames& out) {
+  out.frames.clear(); out.poses.clear();
+  for (uint64_t f = f0; f < f1; ++f) {
+    float T[16];
+    if (int rc = scn_sens_frame_meta(s, f, T, nullptr, nullptr, nullptr, nullptr)) return rc;
+    if (T[0] == -INFINITY) continue;
+    out.frames.push_back(f); out.poses.insert(out.poses.end(), T, T + 16);
+  }
+  return SCN_OK;
+}
+
+int scn::sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, size_t n_px, uint8_t* scratch, uint8_t* out) {
+  if (int rc = scn_sens_frame_color_rgb8(s, frame, scratch)) return rc;
+  for (size_t p = 0; p < n_px; ++p) {
+    const int32_t q = lut[p]; uint8_t* o = out + 3 * p;
+    if (q >= 0) { o[0] = scratch[3 * (size_t)q]; o[1] = scratch[3 * (size_t)q + 1]; o[2] = scratch[3 * (size_t)q + 2]; } else o[0] = o[1] = o[2] = 0;
+  }
+  return SCN_OK;
+}
