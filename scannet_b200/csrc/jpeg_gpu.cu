@@ -429,6 +429,9 @@ void parse_frame(const uint8_t* d, size_t n, uint32_t want_w, uint32_t want_h, P
         if (!f.ch[i] || f.ch[i] > 2 || !f.cv[i] || f.cv[i] > 2 || f.tq[i] > 3) return;
         hmax = std::max(hmax, (int)f.ch[i]); vmax = std::max(vmax, (int)f.cv[i]);
       }
+      // a one-component frame is one non-interleaved scan whatever its sampling factors say: one block per MCU, ceil(W / 8)
+      // blocks per row (T.81 A.2.2; jpeg.cpp and stb read it so)
+      if (nc == 1) f.ch[0] = f.cv[0] = 1, hmax = vmax = 1;
       if (f.ch[0] != hmax || f.cv[0] != vmax) return;             // luma carries the full resolution
       for (int i = 1; i < nc; ++i) if (f.ch[i] != 1 || f.cv[i] != 1) return;
       f.hmax = (unsigned char)hmax; f.vmax = (unsigned char)vmax;
