@@ -26,6 +26,24 @@ def test_filter_matches_cpu_restatement(built, sd, sr, wh):
     assert np.abs(g[~inv] - raw[~inv]).max() < 0.2
 
 
+@pytest.mark.parametrize("sd,sr,wh", [(2.0, 0.05, (160, 120)), (2.0, 0.1, (97, 61)), (1.0, 0.02, (64, 48)), (3.5, 0.05, (80, 60)),
+                                      (4.0, 0.05, (80, 60)), (0.1, 0.05, (80, 60))])
+def test_filter_matches_float64(built, sd, sr, wh):
+    """Against the float64 statement of the filter (tests/tsdf_reference.py:bilateral_f64), which shares no arithmetic with
+    the kernel or the oracle.  Bound from the number of taps n = (2r + 1)^2: binary32 sums of n weights and n weighted depths
+    (n roundings each) and weights within ~4 ulp (expf, the double exp rounded to float, the product) put the weighted
+    mean within (2n + 8) ulp of the largest depth of the window."""
+    import tsdf_reference as tref
+    D, _, _, _ = synth.make_frames(1, seed=5, width=wh[0], height=wh[1], noise_mm=4.0, drop=0.08, with_color=False)
+    g = tsdf.bilateral_filter(D[0], 1000.0, sd, sr)
+    ref, taps = tref.bilateral_f64(D[0], 1000.0, sd, sr)
+    inv = np.isinf(ref)
+    assert (np.isinf(g) == inv).all() and (g[inv] == -np.inf).all()
+    err = np.abs(g[~inv].astype(np.float64) - ref[~inv])
+    assert err.max() <= (2 * taps + 8) * 2.0 ** -24 * np.abs(ref[~inv]).max(), err.max()
+    assert (err > 0).any()                                     # the comparison is not with itself
+
+
 def test_fused_filter_path_bit_exact_given_filtered_depth(built):
     p = tsdf.default_params(width=128, height=96, max_blocks=1 << 15, hash_slots=1 << 17, batch_frames=3,
                             depth_filter=1, depth_sigma_d=2.0, depth_sigma_r=0.05)
