@@ -21,16 +21,15 @@
 #include <cstring>
 #include <vector>
 
-#include "jpeg_tables.h"
+#include "jpeg_common.h"
 #include "scn_common.h"
 
 namespace {
 
-using scn_jpeg::HuffTab;
-using scn_jpeg::kFastBits;
-const uint8_t* const kZig = scn_jpeg::kZigHost;
+using namespace scn_jpeg;
 
-struct Comp { int id = 0, h = 1, v = 1, tq = 0, td = 0, ta = 0, dc_pred = 0, x = 0, y = 0, w2 = 0, h2 = 0, coeff_w = 0; std::vector<uint8_t> data; std::vector<short> coeff; };
+// decoding state of one component: planes (and progressive coefficients) sized from the frame header
+struct Comp { int dc_pred = 0, x = 0, y = 0, w2 = 0, h2 = 0, coeff_w = 0; std::vector<uint8_t> data; std::vector<short> coeff; };
 
 struct Bits {
   const uint8_t* p; size_t n, pos; uint32_t buf = 0; int cnt = 0; bool hit_marker = false;
@@ -62,9 +61,6 @@ struct Bits {
   void reset() { buf = 0; cnt = 0; hit_marker = false; }
 };
 
-inline int extend(int v, int t) { return v < (1 << (t - 1)) ? v - (1 << t) + 1 : v; }
-inline uint8_t clamp8(int x) { return (unsigned)x > 255u ? (x < 0 ? 0 : 255) : (uint8_t)x; }
-
 // AVX2 clones of the two hot loops, picked at load time.  (SCN_NO_TARGET_CLONES: ThreadSanitizer builds — the ifunc
 // resolver would run before the sanitizer runtime is up.)
 #ifdef SCN_NO_TARGET_CLONES
@@ -72,25 +68,6 @@ inline uint8_t clamp8(int x) { return (unsigned)x > 255u ? (x < 0 ? 0 : 255) : (
 #else
 #define SCN_CLONES __attribute__((target_clones("avx2", "default")))
 #endif
-#define F2F(x) ((int)(((x) * 4096 + 0.5)))
-#define IDCT_1D(s0, s1, s2, s3, s4, s5, s6, s7)                                      \
-  int t0, t1, t2, t3, p1, p2, p3, p4, p5, x0, x1, x2, x3;                            \
-  p2 = s2; p3 = s6;                                                                  \
-  p1 = (p2 + p3) * F2F(0.5411961f);                                                  \
-  t2 = p1 + p3 * F2F(-1.847759065f);                                                 \
-  t3 = p1 + p2 * F2F(0.765366865f);                                                  \
-  p2 = s0; p3 = s4;                                                                  \
-  t0 = (p2 + p3) << 12; t1 = (p2 - p3) << 12;                                        \
-  x0 = t0 + t3; x3 = t0 - t3; x1 = t1 + t2; x2 = t1 - t2;                            \
-  t0 = s7; t1 = s5; t2 = s3; t3 = s1;                                                \
-  p3 = t0 + t2; p4 = t1 + t3; p1 = t0 + t3; p2 = t1 + t2;                            \
-  p5 = (p3 + p4) * F2F(1.175875602f);                                                \
-  t0 = t0 * F2F(0.298631336f); t1 = t1 * F2F(2.053119869f);                          \
-  t2 = t2 * F2F(3.072711026f); t3 = t3 * F2F(1.501321110f);                          \
-  p1 = p5 + p1 * F2F(-0.899976223f); p2 = p5 + p2 * F2F(-2.562915447f);              \
-  p3 = p3 * F2F(-1.961570560f); p4 = p4 * F2F(-0.390180644f);                        \
-  t3 += p1 + p4; t2 += p2 + p3; t1 += p2 + p4; t0 += p1 + p3;
-
 // The same arithmetic, eight columns (then eight rows) at a time in 32-bit lanes: every add, multiply (low 32 bits) and shift
 // is the scalar one, so the bytes are identical.  The column shortcut for all-zero AC terms is not needed: with only s0 set the
 // general formula gives (s0 << 12 + 512) >> 10 == s0 << 2 as well.
@@ -254,16 +231,6 @@ const uint8_t* up_generic(uint8_t* out, const uint8_t* in, int w, int hs) {
   return out;
 }
 
-#define FIX20(x) (((int)((x) * 4096.0f + 0.5f)) << 8)
-inline void ycc_to_rgb(uint8_t* out, int y, int cbv, int crv) {
-  const int yf = (y << 20) + (1 << 19), cr = crv - 128, cb = cbv - 128;
-  int r = yf + cr * FIX20(1.40200f);
-  int g = yf + (cr * -FIX20(0.71414f)) + ((cb * -FIX20(0.34414f)) & 0xffff0000);
-  int b = yf + cb * FIX20(1.77200f);
-  r >>= 20; g >>= 20; b >>= 20;
-  out[0] = clamp8(r); out[1] = clamp8(g); out[2] = clamp8(b);
-}
-
 #if defined(__x86_64__)
 // eight pixels per step in 32-bit lanes, the same fixed-point arithmetic; saturating packs == clamp8; a byte shuffle interleaves
 __attribute__((target("avx2"))) static int ycc_row_to_rgb_avx2(uint8_t* o, const uint8_t* y, const uint8_t* cb, const uint8_t* cr, int W) {
@@ -293,18 +260,26 @@ void ycc_row_to_rgb(uint8_t* o, const uint8_t* y, const uint8_t* cb, const uint8
 #if defined(__x86_64__)
   if (use_avx2()) i = ycc_row_to_rgb_avx2(o, y, cb, cr, W);
 #endif
-  for (; i < W; ++i) ycc_to_rgb(o + 3 * i, y[i], cb[i], cr[i]);
+  for (; i < W; ++i) { const unsigned c = ycc_to_rgb(y[i], cb[i], cr[i]); o[3 * i] = (uint8_t)c; o[3 * i + 1] = (uint8_t)(c >> 8); o[3 * i + 2] = (uint8_t)(c >> 16); }
 }
 
 }  // namespace
 
 namespace scn {
 
+// error code and text of each refusal of the marker parser, in the order of scn_jpeg::Parse from kTruncated on
+static const struct { int code; const char* text; } kRefusal[] = {
+    {SCN_ERR_FORMAT, "truncated JPEG"}, {SCN_ERR_FORMAT, "bad JPEG segment length"},
+    {SCN_ERR_UNSUPPORTED, "16-bit quantisation tables are not supported (as in stb_image)"}, {SCN_ERR_FORMAT, "bad DQT"},
+    {SCN_ERR_FORMAT, "bad DHT"}, {SCN_ERR_FORMAT, "bad code lengths"}, {SCN_ERR_FORMAT, "bad DRI"}, {SCN_ERR_UNSUPPORTED, "only 8-bit JPEG"},
+    {SCN_ERR_FORMAT, "bad SOF"}, {SCN_ERR_FORMAT, nullptr /* kBadSize: formatted below */}, {SCN_ERR_FORMAT, "bad SOF component"},
+    {SCN_ERR_FORMAT, "SOS before SOF"}, {SCN_ERR_FORMAT, "bad SOS"}, {SCN_ERR_FORMAT, "bad SOS component"},
+    {SCN_ERR_FORMAT, "scan references a missing table"}};
+static_assert(sizeof(kRefusal) / sizeof(kRefusal[0]) == kMissingTable - kTruncated + 1, "one entry per refusal");
+
 int jpeg_decode_rgb8(const uint8_t* d, size_t n, uint32_t want_w, uint32_t want_h, uint8_t* out) {
   if (n < 4 || d[0] != 0xFF || d[1] != 0xD8) return fail(SCN_ERR_FORMAT, "not a JPEG (no SOI)");
-  uint8_t quant[4][64]; bool have_q[4] = {false, false, false, false};
-  HuffTab hdc[4], hac[4];
-  for (int i = 0; i < 4; ++i) hdc[i].present = hac[i].present = 0;
+  Header hd(want_w, want_h);
   Comp comp[3];
   // plane buffers are leased from the calling thread and handed back on every exit path: a decoder pool of 64 threads doing
   // a 460 KB allocation + page faults per frame serialised on the process's memory map (31 ms per 128-frame chunk instead of 7)
@@ -313,247 +288,188 @@ int jpeg_decode_rgb8(const uint8_t* d, size_t n, uint32_t want_w, uint32_t want_
     Comp* c; std::vector<uint8_t>* t; int n;
     PlaneLease(Comp* c_, std::vector<uint8_t>* t_, int n_) : c(c_), t(t_), n(n_) { for (int i = 0; i < n; ++i) c[i].data.swap(t[i]); }
     ~PlaneLease() { for (int i = 0; i < n; ++i) c[i].data.swap(t[i]); }
-  } lease(comp, tl_planes, 3); int ncomp = 0, W = 0, H = 0, hmax = 1, vmax = 1, mcux = 0, mcuy = 0, restart = 0;
-  bool progressive = false;
-  bool have_frame = false;
-  size_t pos = 2;
-  for (;;) {
-    while (pos < n && d[pos] != 0xFF) ++pos;
-    while (pos < n && d[pos] == 0xFF) ++pos;
-    if (pos >= n) break;
-    const int m = d[pos++];
-    if (m == 0xD9) break;
-    if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) continue;
-    if (pos + 2 > n) return fail(SCN_ERR_FORMAT, "truncated JPEG");
-    const size_t len = ((size_t)d[pos] << 8) | d[pos + 1];
-    if (len < 2 || pos + len > n) return fail(SCN_ERR_FORMAT, "bad JPEG segment length");
-    const uint8_t* s = d + pos + 2; size_t sl = len - 2;
-    if (m == 0xDB) {
-      while (sl > 0) {
-        const int pq = s[0] >> 4, tq = s[0] & 15;
-        if (pq != 0) return fail(SCN_ERR_UNSUPPORTED, "16-bit quantisation tables are not supported (as in stb_image)");
-        if (tq > 3 || sl < 65) return fail(SCN_ERR_FORMAT, "bad DQT");
-        for (int i = 0; i < 64; ++i) quant[tq][kZig[i]] = s[1 + i];
-        have_q[tq] = true; s += 65; sl -= 65;
-      }
-    } else if (m == 0xC4) {
-      while (sl > 0) {
-        if (sl < 17) return fail(SCN_ERR_FORMAT, "bad DHT");
-        const int tc = s[0] >> 4, th = s[0] & 15; int tot = 0;
-        for (int i = 0; i < 16; ++i) tot += s[1 + i];
-        if (tc > 1 || th > 3 || tot > 256 || sl < (size_t)(17 + tot)) return fail(SCN_ERR_FORMAT, "bad DHT");
-        if (!(tc ? hac[th] : hdc[th]).build(s + 1, s + 17, tot)) return fail(SCN_ERR_FORMAT, "bad code lengths");
-        if (tc) hac[th].build_fast_ac();
-        s += 17 + tot; sl -= 17 + tot;
-      }
-    } else if (m == 0xDD) { if (sl < 2) return fail(SCN_ERR_FORMAT, "bad DRI"); restart = (s[0] << 8) | s[1]; }
-    else if (m == 0xC0 || m == 0xC1 || m == 0xC2) {
-      progressive = m == 0xC2;
-      if (sl < 6 || s[0] != 8) return fail(SCN_ERR_UNSUPPORTED, "only 8-bit JPEG");
-      H = (s[1] << 8) | s[2]; W = (s[3] << 8) | s[4]; ncomp = s[5];
-      if ((ncomp != 1 && ncomp != 3) || sl < (size_t)(6 + 3 * ncomp) || W == 0 || H == 0) return fail(SCN_ERR_FORMAT, "bad SOF");
-      // the container's header fixes the frame size: refuse before any plane is sized from in-stream values
-      if ((uint32_t)W != want_w || (uint32_t)H != want_h) return fail(SCN_ERR_FORMAT, "JPEG is %dx%d, header says %ux%u", W, H, want_w, want_h);
-      for (int i = 0; i < ncomp; ++i) {
-        comp[i].id = s[6 + 3 * i]; comp[i].h = s[7 + 3 * i] >> 4; comp[i].v = s[7 + 3 * i] & 15; comp[i].tq = s[8 + 3 * i];
-        if (!comp[i].h || comp[i].h > 4 || !comp[i].v || comp[i].v > 4 || comp[i].tq > 3) return fail(SCN_ERR_FORMAT, "bad SOF component");
-        hmax = std::max(hmax, comp[i].h); vmax = std::max(vmax, comp[i].v);
-      }
+  } lease(comp, tl_planes, 3);
+  int mcux = 0, mcuy = 0, sized_for = 0;             // sized_for: the frame header (by count) the planes were last sized for
+  Scan sc;
+  for (size_t pos = 2;;) {
+    const Parse pr = parse_header(d, n, pos, hd, sc);
+    if (pr == kBadSize) return fail(SCN_ERR_FORMAT, "JPEG is %dx%d, header says %ux%u", hd.W, hd.H, want_w, want_h);
+    if (pr != kScan && pr != kEnd) return fail(kRefusal[pr - kTruncated].code, "%s", kRefusal[pr - kTruncated].text);
+    const int ncomp = hd.ncomp, W = hd.W, H = hd.H, hmax = hd.hmax, vmax = hd.vmax;
+    const bool progressive = hd.sof == 0xC2;
+    if (hd.n_sof != sized_for) {                       // a new frame header: (re)size and clear the planes
+      sized_for = hd.n_sof;
       mcux = (W + 8 * hmax - 1) / (8 * hmax); mcuy = (H + 8 * vmax - 1) / (8 * vmax);
       for (int i = 0; i < ncomp; ++i) {
-        comp[i].x = (W * comp[i].h + hmax - 1) / hmax; comp[i].y = (H * comp[i].v + vmax - 1) / vmax;
-        comp[i].w2 = mcux * comp[i].h * 8; comp[i].h2 = mcuy * comp[i].v * 8;
+        const FrameComp& f = hd.comp[i];
+        comp[i].x = (W * f.h + hmax - 1) / hmax; comp[i].y = (H * f.v + vmax - 1) / vmax;
+        comp[i].w2 = mcux * f.h * 8; comp[i].h2 = mcuy * f.v * 8;
         comp[i].data.assign((size_t)comp[i].w2 * comp[i].h2 + 15, 0);
         if (progressive) { comp[i].coeff_w = comp[i].w2 >> 3; comp[i].coeff.assign((size_t)comp[i].coeff_w * (comp[i].h2 >> 3) * 64, 0); }
       }
-      have_frame = true;
-    } else if (m == 0xDA) {
-      if (!have_frame) return fail(SCN_ERR_FORMAT, "SOS before SOF");
-      if (sl < 1) return fail(SCN_ERR_FORMAT, "bad SOS");
-      const int ns = s[0];
-      if (ns < 1 || ns > ncomp || sl < (size_t)(1 + 2 * ns + 3)) return fail(SCN_ERR_FORMAT, "bad SOS");
-      int order[3];
-      for (int i = 0; i < ns; ++i) {
-        int which = -1;
-        for (int c = 0; c < ncomp; ++c) if (comp[c].id == s[1 + 2 * i]) which = c;
-        if (which < 0) return fail(SCN_ERR_FORMAT, "bad SOS component");
-        comp[which].td = s[2 + 2 * i] >> 4; comp[which].ta = s[2 + 2 * i] & 15;
-        if (comp[which].td > 3 || comp[which].ta > 3 || !have_q[comp[which].tq]) return fail(SCN_ERR_FORMAT, "scan references a missing table");
-        order[i] = which;
+    }
+    if (pr == kEnd) break;
+    const int ns = sc.ns, spec_start = sc.ss, spec_end = sc.se, succ_high = sc.ah, succ_low = sc.al, restart = hd.restart;
+    const int* order = sc.comp;
+    Bits br{d, n, sc.data};
+    for (int c = 0; c < ncomp; ++c) comp[c].dc_pred = 0;
+    int todo = restart ? restart : 0x7fffffff;
+    short blk[64];
+    auto decode_block = [&](int kc, int bx, int by) -> bool {
+      Comp& c = comp[kc]; const FrameComp& f = hd.comp[kc];
+      memset(blk, 0, sizeof(blk));
+      const int t = br.decode(hd.dc[f.td]);
+      if (t < 0 || t > 16) return false;
+      const int diff = t ? extend(br.get(t), t) : 0;
+      c.dc_pred += diff;
+      const uint8_t* q = hd.quant[f.tq];
+      blk[0] = (short)(c.dc_pred * q[0]);
+      const HuffTab& ha = hd.ac[f.ta];
+      for (int k = 1; k < 64;) {
+        if (br.cnt < 16) br.fill();
+        const int fa = ha.fast_ac[br.buf >> (32 - kFastBits)];
+        if (fa) {                                             // short code + small coefficient in one lookup
+          k += (fa >> 4) & 15;
+          const int used = fa & 15;
+          br.buf <<= used; br.cnt -= used;
+          const int z = kZig[k++];
+          blk[z] = (short)((fa >> 8) * q[z]);
+          continue;
+        }
+        const int rs = br.decode(ha);
+        if (rs < 0) return false;
+        const int sz = rs & 15, r = rs >> 4;
+        if (sz == 0) { if (rs != 0xF0) break; k += 16; }
+        else { k += r; const int z = kZig[k++]; blk[z] = (short)(extend(br.get(sz), sz) * q[z]); }
       }
-      // spectral selection / successive approximation (stb_image.h:2665-2702)
-      const int spec_start = s[1 + 2 * ns], spec_end_raw = s[2 + 2 * ns], succ_high = s[3 + 2 * ns] >> 4, succ_low = s[3 + 2 * ns] & 15;
-      int spec_end = spec_end_raw;
-      if (progressive) {
-        if (spec_start > 63 || spec_end > 63 || spec_start > spec_end || succ_high > 13 || succ_low > 13) return fail(SCN_ERR_FORMAT, "bad SOS");
-      } else {
-        if (spec_start != 0 || succ_high != 0 || succ_low != 0) return fail(SCN_ERR_FORMAT, "bad SOS");
-        spec_end = 63;
-      }
-      for (int i = 0; i < ns; ++i) {
-        const Comp& c = comp[order[i]];
-        const bool need_dc = !progressive || spec_start == 0, need_ac = !progressive || spec_start != 0;
-        if ((need_dc && !hdc[c.td].present) || (need_ac && !hac[c.ta].present)) return fail(SCN_ERR_FORMAT, "scan references a missing table");
-      }
-      Bits br{d, n, pos + len};
-      for (int c = 0; c < ncomp; ++c) comp[c].dc_pred = 0;
-      int todo = restart ? restart : 0x7fffffff;
-      short blk[64];
-      auto decode_block = [&](Comp& c, int bx, int by) -> bool {
-        memset(blk, 0, sizeof(blk));
-        const int t = br.decode(hdc[c.td]);
+      idct8x8(c.data.data() + (size_t)c.w2 * by * 8 + (size_t)bx * 8, c.w2, blk);
+      return true;
+    };
+    int eob_run = 0;
+    // progressive passes write into the persistent coefficient blocks (stb_image.h:1771-1913); same arithmetic, in shorts
+    auto prog_dc = [&](int kc, short* data) -> bool {
+      if (spec_end != 0) return false;                                     // "can't merge dc and ac"
+      if (succ_high == 0) {
+        memset(data, 0, 64 * sizeof(short));
+        const int t = br.decode(hd.dc[hd.comp[kc].td]);
         if (t < 0 || t > 16) return false;
         const int diff = t ? extend(br.get(t), t) : 0;
-        c.dc_pred += diff;
-        blk[0] = (short)(c.dc_pred * quant[c.tq][0]);
-        const HuffTab& ha = hac[c.ta];
-        for (int k = 1; k < 64;) {
+        comp[kc].dc_pred += diff;
+        data[0] = (short)(comp[kc].dc_pred << succ_low);
+      } else if (br.get(1)) data[0] += (short)(1 << succ_low);
+      return true;
+    };
+    auto prog_ac = [&](int kc, short* data) -> bool {
+      if (spec_start == 0) return false;
+      const HuffTab& ha = hd.ac[hd.comp[kc].ta];
+      if (succ_high == 0) {
+        const int shift = succ_low;
+        if (eob_run) { --eob_run; return true; }
+        int k = spec_start;
+        do {
           if (br.cnt < 16) br.fill();
           const int fa = ha.fast_ac[br.buf >> (32 - kFastBits)];
-          if (fa) {                                             // short code + small coefficient in one lookup
+          if (fa) {
             k += (fa >> 4) & 15;
             const int used = fa & 15;
             br.buf <<= used; br.cnt -= used;
-            const int z = kZig[k++];
-            blk[z] = (short)((fa >> 8) * quant[c.tq][z]);
-            continue;
+            data[kZig[k++]] = (short)((fa >> 8) << shift);
+          } else {
+            const int rs = br.decode(ha);
+            if (rs < 0) return false;
+            const int sz = rs & 15, r = rs >> 4;
+            if (sz == 0) {
+              if (r < 15) { eob_run = 1 << r; if (r) eob_run += br.get(r); --eob_run; break; }
+              k += 16;
+            } else { k += r; data[kZig[k++]] = (short)(extend(br.get(sz), sz) << shift); }
           }
-          const int rs = br.decode(ha);
-          if (rs < 0) return false;
-          const int sz = rs & 15, r = rs >> 4;
-          if (sz == 0) { if (rs != 0xF0) break; k += 16; }
-          else { k += r; const int z = kZig[k++]; blk[z] = (short)(extend(br.get(sz), sz) * quant[c.tq][z]); }
-        }
-        idct8x8(c.data.data() + (size_t)c.w2 * by * 8 + (size_t)bx * 8, c.w2, blk);
-        return true;
-      };
-      int eob_run = 0;
-      // progressive passes write into the persistent coefficient blocks (stb_image.h:1771-1913); same arithmetic, in shorts
-      auto prog_dc = [&](Comp& c, short* data) -> bool {
-        if (spec_end != 0) return false;                                     // "can't merge dc and ac"
-        if (succ_high == 0) {
-          memset(data, 0, 64 * sizeof(short));
-          const int t = br.decode(hdc[c.td]);
-          if (t < 0 || t > 16) return false;
-          const int diff = t ? extend(br.get(t), t) : 0;
-          c.dc_pred += diff;
-          data[0] = (short)(c.dc_pred << succ_low);
-        } else if (br.get(1)) data[0] += (short)(1 << succ_low);
-        return true;
-      };
-      auto prog_ac = [&](Comp& c, short* data) -> bool {
-        if (spec_start == 0) return false;
-        const HuffTab& ha = hac[c.ta];
-        if (succ_high == 0) {
-          const int shift = succ_low;
-          if (eob_run) { --eob_run; return true; }
+        } while (k <= spec_end);
+      } else {
+        const short bit = (short)(1 << succ_low);
+        auto refine = [&](short* p) { if (br.get(1) && (*p & bit) == 0) { if (*p > 0) *p += bit; else *p -= bit; } };
+        if (eob_run) {
+          --eob_run;
+          for (int k = spec_start; k <= spec_end; ++k) { short* p = &data[kZig[k]]; if (*p != 0) refine(p); }
+        } else {
           int k = spec_start;
           do {
-            if (br.cnt < 16) br.fill();
-            const int fa = ha.fast_ac[br.buf >> (32 - kFastBits)];
-            if (fa) {
-              k += (fa >> 4) & 15;
-              const int used = fa & 15;
-              br.buf <<= used; br.cnt -= used;
-              data[kZig[k++]] = (short)((fa >> 8) << shift);
+            const int rs = br.decode(ha);
+            if (rs < 0) return false;
+            int sz = rs & 15, r = rs >> 4;
+            if (sz == 0) {
+              if (r < 15) { eob_run = (1 << r) - 1; if (r) eob_run += br.get(r); r = 64; }
             } else {
-              const int rs = br.decode(ha);
-              if (rs < 0) return false;
-              const int sz = rs & 15, r = rs >> 4;
-              if (sz == 0) {
-                if (r < 15) { eob_run = 1 << r; if (r) eob_run += br.get(r); --eob_run; break; }
-                k += 16;
-              } else { k += r; data[kZig[k++]] = (short)(extend(br.get(sz), sz) << shift); }
+              if (sz != 1) return false;
+              sz = br.get(1) ? bit : -bit;
+            }
+            while (k <= spec_end) {
+              short* p = &data[kZig[k++]];
+              if (*p != 0) refine(p);
+              else { if (r == 0) { *p = (short)sz; break; } --r; }
             }
           } while (k <= spec_end);
-        } else {
-          const short bit = (short)(1 << succ_low);
-          auto refine = [&](short* p) { if (br.get(1) && (*p & bit) == 0) { if (*p > 0) *p += bit; else *p -= bit; } };
-          if (eob_run) {
-            --eob_run;
-            for (int k = spec_start; k <= spec_end; ++k) { short* p = &data[kZig[k]]; if (*p != 0) refine(p); }
-          } else {
-            int k = spec_start;
-            do {
-              const int rs = br.decode(ha);
-              if (rs < 0) return false;
-              int sz = rs & 15, r = rs >> 4;
-              if (sz == 0) {
-                if (r < 15) { eob_run = (1 << r) - 1; if (r) eob_run += br.get(r); r = 64; }
-              } else {
-                if (sz != 1) return false;
-                sz = br.get(1) ? bit : -bit;
-              }
-              while (k <= spec_end) {
-                short* p = &data[kZig[k++]];
-                if (*p != 0) refine(p);
-                else { if (r == 0) { *p = (short)sz; break; } --r; }
-              }
-            } while (k <= spec_end);
-          }
-        }
-        return true;
-      };
-      auto handle_restart = [&]() {
-        if (--todo <= 0) {
-          eob_run = 0;
-          // byte-align, expect RSTn
-          br.reset();
-          size_t q = br.pos;
-          while (q + 1 < n && !(d[q] == 0xFF && d[q + 1] >= 0xD0 && d[q + 1] <= 0xD7)) { if (d[q] == 0xFF && d[q + 1] != 0 && d[q + 1] != 0xFF) return false; ++q; }
-          if (q + 1 >= n) return false;
-          br.pos = q + 2;
-          for (int c = 0; c < ncomp; ++c) comp[c].dc_pred = 0;
-          todo = restart ? restart : 0x7fffffff;
-        }
-        return true;
-      };
-      bool ended = false;
-      auto one_block = [&](Comp& c, int bx, int by) -> bool {
-        if (!progressive) return decode_block(c, bx, by);
-        short* data = c.coeff.data() + 64 * ((size_t)bx + (size_t)by * c.coeff_w);
-        return (ns > 1 || spec_start == 0) ? prog_dc(c, data) : prog_ac(c, data);        // interleaved progressive scans are DC scans
-      };
-      if (ns == 1) {
-        Comp& c = comp[order[0]];
-        const int bw = (c.x + 7) >> 3, bh = (c.y + 7) >> 3;
-        for (int j = 0; j < bh && !ended; ++j) for (int i = 0; i < bw; ++i) {
-          if (!one_block(c, i, j)) return fail(SCN_ERR_FORMAT, "bad huffman code");
-          if (!handle_restart()) { ended = true; break; }
-        }
-      } else {
-        for (int j = 0; j < mcuy && !ended; ++j) for (int i = 0; i < mcux; ++i) {
-          for (int k = 0; k < ns; ++k) { Comp& c = comp[order[k]];
-            for (int y = 0; y < c.v; ++y) for (int x = 0; x < c.h; ++x)
-              if (!one_block(c, i * c.h + x, j * c.v + y)) return fail(SCN_ERR_FORMAT, "bad huffman code"); }
-          if (!handle_restart()) { ended = true; break; }
         }
       }
-      // continue the marker scan after the entropy-coded data
-      pos = br.pos;
-      while (pos + 1 < n && !(d[pos] == 0xFF && d[pos + 1] != 0 && !(d[pos + 1] >= 0xD0 && d[pos + 1] <= 0xD7) && d[pos + 1] != 0xFF)) ++pos;
-      continue;
+      return true;
+    };
+    auto handle_restart = [&]() {
+      if (--todo <= 0) {
+        eob_run = 0;
+        // byte-align, expect RSTn
+        br.reset();
+        size_t q = br.pos;
+        while (q + 1 < n && !(d[q] == 0xFF && d[q + 1] >= 0xD0 && d[q + 1] <= 0xD7)) { if (d[q] == 0xFF && d[q + 1] != 0 && d[q + 1] != 0xFF) return false; ++q; }
+        if (q + 1 >= n) return false;
+        br.pos = q + 2;
+        for (int c = 0; c < ncomp; ++c) comp[c].dc_pred = 0;
+        todo = restart ? restart : 0x7fffffff;
+      }
+      return true;
+    };
+    bool ended = false;
+    auto one_block = [&](int kc, int bx, int by) -> bool {
+      if (!progressive) return decode_block(kc, bx, by);
+      short* data = comp[kc].coeff.data() + 64 * ((size_t)bx + (size_t)by * comp[kc].coeff_w);
+      return (ns > 1 || spec_start == 0) ? prog_dc(kc, data) : prog_ac(kc, data);        // interleaved progressive scans are DC scans
+    };
+    if (ns == 1) {
+      const Comp& c = comp[order[0]];
+      const int bw = (c.x + 7) >> 3, bh = (c.y + 7) >> 3;
+      for (int j = 0; j < bh && !ended; ++j) for (int i = 0; i < bw; ++i) {
+        if (!one_block(order[0], i, j)) return fail(SCN_ERR_FORMAT, "bad huffman code");
+        if (!handle_restart()) { ended = true; break; }
+      }
+    } else {
+      for (int j = 0; j < mcuy && !ended; ++j) for (int i = 0; i < mcux; ++i) {
+        for (int k = 0; k < ns; ++k) { const FrameComp& f = hd.comp[order[k]];
+          for (int y = 0; y < f.v; ++y) for (int x = 0; x < f.h; ++x)
+            if (!one_block(order[k], i * f.h + x, j * f.v + y)) return fail(SCN_ERR_FORMAT, "bad huffman code"); }
+        if (!handle_restart()) { ended = true; break; }
+      }
     }
-    pos += len;
+    // continue the marker scan after the entropy-coded data
+    pos = br.pos;
+    while (pos + 1 < n && !(d[pos] == 0xFF && d[pos + 1] != 0 && !(d[pos + 1] >= 0xD0 && d[pos + 1] <= 0xD7) && d[pos + 1] != 0xFF)) ++pos;
   }
-  if (!have_frame) return fail(SCN_ERR_FORMAT, "no frame in JPEG");
-  if (progressive) {                                                          // stbi__jpeg_finish: dequantise (in shorts) + IDCT of every real block
+  if (!hd.sof) return fail(SCN_ERR_FORMAT, "no frame in JPEG");
+  const int ncomp = hd.ncomp, W = hd.W, H = hd.H, hmax = hd.hmax, vmax = hd.vmax;
+  if (hd.sof == 0xC2) {                                                       // stbi__jpeg_finish: dequantise (in shorts) + IDCT of every real block
     for (int k = 0; k < ncomp; ++k) {
       Comp& c = comp[k];
-      if (!have_q[c.tq]) return fail(SCN_ERR_FORMAT, "scan references a missing table");
+      if (!hd.have_q[hd.comp[k].tq]) return fail(SCN_ERR_FORMAT, "scan references a missing table");
+      const uint8_t* q = hd.quant[hd.comp[k].tq];
       const int bw = (c.x + 7) >> 3, bh = (c.y + 7) >> 3;
       for (int j = 0; j < bh; ++j) for (int i = 0; i < bw; ++i) {
         short* data = c.coeff.data() + 64 * ((size_t)i + (size_t)j * c.coeff_w);
-        for (int q = 0; q < 64; ++q) data[q] = (short)(data[q] * quant[c.tq][q]);
+        for (int z = 0; z < 64; ++z) data[z] = (short)(data[z] * q[z]);
         idct8x8(c.data.data() + (size_t)c.w2 * j * 8 + (size_t)i * 8, c.w2, data);
       }
     }
   }
-  if ((uint32_t)W != want_w || (uint32_t)H != want_h) return fail(SCN_ERR_FORMAT, "JPEG is %dx%d, header says %ux%u", W, H, want_w, want_h);
   // up-sample + colour convert, row by row (stb_image.h:3166-3250)
   struct Res { int hs, vs, ystep, wl, ypos; const uint8_t *l0, *l1; std::vector<uint8_t> buf; } rs[3];
   for (int k = 0; k < ncomp; ++k) {
-    rs[k].hs = hmax / comp[k].h; rs[k].vs = vmax / comp[k].v; rs[k].ystep = rs[k].vs >> 1;
+    rs[k].hs = hmax / hd.comp[k].h; rs[k].vs = vmax / hd.comp[k].v; rs[k].ystep = rs[k].vs >> 1;
     rs[k].wl = (W + rs[k].hs - 1) / rs[k].hs; rs[k].ypos = 0; rs[k].l0 = rs[k].l1 = comp[k].data.data();
     rs[k].buf.assign((size_t)W + 16 + 8 * hmax, 0);
   }

@@ -24,16 +24,13 @@
 #include <thread>
 #include <vector>
 
-#include "jpeg_tables.h"
+#include "jpeg_common.h"
 #include "scn_common.h"
 #include "stage_pool.h"
 
-namespace scn { int jpeg_decode_rgb8(const uint8_t* d, size_t n, uint32_t want_w, uint32_t want_h, uint8_t* out); }
-
 namespace {
 
-using scn_jpeg::HuffTab;
-using scn_jpeg::kFastBits;
+using namespace scn_jpeg;
 
 struct TableSet { HuffTab dc[2], ac[2]; uint8_t quant[4][64]; uint8_t have_q[4]; uint8_t pad[12]; };
 static_assert(sizeof(TableSet) % 16 == 0, "TableSet is copied to shared memory in 16-byte pieces");
@@ -53,9 +50,7 @@ struct FrameDesc {
 };
 static_assert(sizeof(FrameDesc) % 8 == 0, "FrameDesc is copied word by word");
 
-__constant__ unsigned char c_zig[64 + 15] = {0,1,8,16,9,2,3,10,17,24,32,25,18,11,4,5,12,19,26,33,40,48,41,34,27,20,13,6,7,14,21,28,35,42,49,56,57,50,43,36,
-                                             29,22,15,23,30,37,44,51,58,59,52,45,38,31,39,46,53,60,61,54,47,55,62,63,
-                                             63,63,63,63,63,63,63,63,63,63,63,63,63,63,63};
+__constant__ unsigned char c_zig[64 + 15] = SCN_JPEG_ZIG;
 
 // MSB-first bit reader over the entropy-coded segment, same bit stream as jpeg.cpp's `Bits` (byte stuffing removed, a marker
 // stops the input: zero bits from then on) - but the stuffing is removed by the WHOLE WARP, 32 raw bytes per step (ballot +
@@ -146,27 +141,6 @@ struct CleanBits {
   }
   __device__ __forceinline__ unsigned end_pos() const { return marker ? marker_pos : raw_pos; }
 };
-__device__ __forceinline__ int jextend(int v, int t) { return v < (1 << (t - 1)) ? v - (1 << t) + 1 : v; }
-__device__ __forceinline__ int clamp8(int x) { return (unsigned)x > 255u ? (x < 0 ? 0 : 255) : x; }
-
-#define F2F(x) ((int)(((x) * 4096 + 0.5)))
-#define IDCT_1D(s0, s1, s2, s3, s4, s5, s6, s7)                                      \
-  int t0, t1, t2, t3, p1, p2, p3, p4, p5, x0, x1, x2, x3;                            \
-  p2 = s2; p3 = s6;                                                                  \
-  p1 = (p2 + p3) * F2F(0.5411961f);                                                  \
-  t2 = p1 + p3 * F2F(-1.847759065f);                                                 \
-  t3 = p1 + p2 * F2F(0.765366865f);                                                  \
-  p2 = s0; p3 = s4;                                                                  \
-  t0 = (p2 + p3) << 12; t1 = (p2 - p3) << 12;                                        \
-  x0 = t0 + t3; x3 = t0 - t3; x1 = t1 + t2; x2 = t1 - t2;                            \
-  t0 = s7; t1 = s5; t2 = s3; t3 = s1;                                                \
-  p3 = t0 + t2; p4 = t1 + t3; p1 = t0 + t3; p2 = t1 + t2;                            \
-  p5 = (p3 + p4) * F2F(1.175875602f);                                                \
-  t0 = t0 * F2F(0.298631336f); t1 = t1 * F2F(2.053119869f);                          \
-  t2 = t2 * F2F(3.072711026f); t3 = t3 * F2F(1.501321110f);                          \
-  p1 = p5 + p1 * F2F(-0.899976223f); p2 = p5 + p2 * F2F(-2.562915447f);              \
-  p3 = p3 * F2F(-1.961570560f); p4 = p4 * F2F(-0.390180644f);                        \
-  t3 += p1 + p4; t2 += p2 + p3; t1 += p2 + p4; t0 += p1 + p3;
 
 enum { JST_OK = 0, JST_UNSUPPORTED = 1, JST_BAD_CODE = 2, JST_BAD_RESTART = 3 };
 
@@ -224,7 +198,7 @@ k_jpeg_entropy_idct(const unsigned char* __restrict__ in, const FrameDesc* __res
           short* blk = s_blk[b];
           const int t = br.decode(hd);
           if (t < 0 || t > 16) { rc = JST_BAD_CODE; break; }
-          const int diff = t ? jextend(br.get(t), t) : 0;
+          const int diff = t ? extend(br.get(t), t) : 0;
           const int dc = (k == 0 ? dc0 : k == 1 ? dc1 : dc2) + diff;
           if (k == 0) dc0 = dc; else if (k == 1) dc1 = dc; else dc2 = dc;
           if (lane == 0) blk[0] = (short)(dc * q[0]);
@@ -241,7 +215,7 @@ k_jpeg_entropy_idct(const unsigned char* __restrict__ in, const FrameDesc* __res
             if (rs < 0) { rc = JST_BAD_CODE; break; }
             const int sz = rs & 15, r = rs >> 4;
             if (sz == 0) { if (rs != 0xF0) break; kk += 16; }
-            else { kk += r; const int z = c_zig[kk++]; const int v = jextend(br.get(sz), sz); if (lane == 0) blk[z] = (short)(v * q[z]); }
+            else { kk += r; const int z = c_zig[kk++]; const int v = extend(br.get(sz), sz); if (lane == 0) blk[z] = (short)(v * q[z]); }
           }
           if (rc != JST_OK) break;
         }
@@ -312,7 +286,6 @@ __device__ __forceinline__ int chroma_at(const unsigned char* P, unsigned w2, un
   const int ta = 3 * nr[i - 1] + fr[i - 1], tb = 3 * nr[i] + fr[i];
   return (x & 1) ? (3 * ta + tb + 8) >> 4 : (3 * tb + ta + 8) >> 4;
 }
-#define FIX20(x) (((int)((x) * 4096.0f + 0.5f)) << 8)
 // one colour pixel (x, y) of a decoded frame as r | g << 8 | b << 16 (jpeg.cpp: the per-row conversion; stb_image.h:3091-3118)
 __device__ __forceinline__ unsigned pixel_rgb(const FrameDesc& f, const unsigned char* pl, int x, int y) {
   const int yy = pl[f.plane_off[0] + (size_t)y * f.w2[0] + x];
@@ -324,12 +297,7 @@ __device__ __forceinline__ unsigned pixel_rgb(const FrameDesc& f, const unsigned
     const int hs = (f.hmax == 2 && f.ch[k] == 1) ? 2 : 1, vs = (f.vmax == 2 && f.cv[k] == 1) ? 2 : 1;
     cc[k - 1] = chroma_at(pl + f.plane_off[k], f.w2[k], f.cy[k], (f.W + hs - 1) >> (hs - 1), hs, vs, x, y);
   }
-  const int yf = (yy << 20) + (1 << 19), cr = cc[1] - 128, cb = cc[0] - 128;
-  int r = yf + cr * FIX20(1.40200f);
-  int g = yf + (cr * -FIX20(0.71414f)) + ((cb * -FIX20(0.34414f)) & 0xffff0000);
-  int b = yf + cb * FIX20(1.77200f);
-  r >>= 20; g >>= 20; b >>= 20;
-  return (unsigned)clamp8(r) | ((unsigned)clamp8(g) << 8) | ((unsigned)clamp8(b) << 16);
+  return ycc_to_rgb(yy, cc[0], cc[1]);
 }
 // grid: (ceil(out_px / 256), n frames).  lut == nullptr: out pixel p = colour pixel p (out_px = W*H); else out pixel p shows
 // colour pixel lut[p] (-1 = none -> black), the depth-registered sampling of the fusion path.
@@ -379,89 +347,43 @@ void parse_frame(const uint8_t* d, size_t n, uint32_t want_w, uint32_t want_h, P
   memset(&f, 0, sizeof(f));
   memset(&ts, 0, sizeof(ts));
   out.table_bytes.clear();
-  f.supported = 0;
   if (n < 4 || n > 0xFFFFFFF0ull || d[0] != 0xFF || d[1] != 0xD8) return;
-  int ids[3] = {0, 0, 0};
-  bool have_frame = false;
-  size_t pos = 2;
-  for (;;) {
-    while (pos < n && d[pos] != 0xFF) ++pos;
-    while (pos < n && d[pos] == 0xFF) ++pos;
-    if (pos >= n) return;
-    const int m = d[pos++];
-    if (m == 0xD9) return;
-    if (m == 0x01 || (m >= 0xD0 && m <= 0xD7)) continue;
-    if (pos + 2 > n) return;
-    const size_t len = ((size_t)d[pos] << 8) | d[pos + 1];
-    if (len < 2 || pos + len > n) return;
-    const uint8_t* s = d + pos + 2; size_t sl = len - 2;
-    if (m == 0xDB) {
-      out.table_bytes.insert(out.table_bytes.end(), d + pos - 1, d + pos + len);
-      while (sl > 0) {
-        const int pq = s[0] >> 4, tq = s[0] & 15;
-        if (pq != 0 || tq > 3 || sl < 65) return;
-        for (int i = 0; i < 64; ++i) ts.quant[tq][scn_jpeg::kZigHost[i]] = s[1 + i];
-        ts.have_q[tq] = 1; s += 65; sl -= 65;
-      }
-    } else if (m == 0xC4) {
-      out.table_bytes.insert(out.table_bytes.end(), d + pos - 1, d + pos + len);
-      while (sl > 0) {
-        if (sl < 17) return;
-        const int tc = s[0] >> 4, th = s[0] & 15; int tot = 0;
-        for (int i = 0; i < 16; ++i) tot += s[1 + i];
-        if (tc > 1 || th > 3 || tot > 256 || sl < (size_t)(17 + tot)) return;
-        if (th > 1) return;                                      // device path: table ids 0-1 (baseline)
-        HuffTab& h = tc ? ts.ac[th] : ts.dc[th];
-        if (!h.build(s + 1, s + 17, tot)) return;
-        if (tc) h.build_fast_ac();
-        s += 17 + tot; sl -= 17 + tot;
-      }
-    } else if (m == 0xDD) { if (sl < 2) return; f.restart = (unsigned)((s[0] << 8) | s[1]); }
-    else if (m == 0xC0 || m == 0xC1) {
-      if (have_frame) return;
-      if (sl < 6 || s[0] != 8) return;
-      const int H = (s[1] << 8) | s[2], W = (s[3] << 8) | s[4], nc = s[5];
-      if ((nc != 1 && nc != 3) || sl < (size_t)(6 + 3 * nc) || (uint32_t)W != want_w || (uint32_t)H != want_h || W == 0 || H == 0) return;
-      f.W = (unsigned short)W; f.H = (unsigned short)H; f.ncomp = (unsigned char)nc;
-      int hmax = 1, vmax = 1;
-      for (int i = 0; i < nc; ++i) {
-        ids[i] = s[6 + 3 * i]; f.ch[i] = s[7 + 3 * i] >> 4; f.cv[i] = s[7 + 3 * i] & 15; f.tq[i] = s[8 + 3 * i];
-        if (!f.ch[i] || f.ch[i] > 2 || !f.cv[i] || f.cv[i] > 2 || f.tq[i] > 3) return;
-        hmax = std::max(hmax, (int)f.ch[i]); vmax = std::max(vmax, (int)f.cv[i]);
-      }
-      // a one-component frame is one non-interleaved scan whatever its sampling factors say: one block per MCU, ceil(W / 8)
-      // blocks per row (T.81 A.2.2; jpeg.cpp and stb read it so)
-      if (nc == 1) f.ch[0] = f.cv[0] = 1, hmax = vmax = 1;
-      if (f.ch[0] != hmax || f.cv[0] != vmax) return;             // luma carries the full resolution
-      for (int i = 1; i < nc; ++i) if (f.ch[i] != 1 || f.cv[i] != 1) return;
-      f.hmax = (unsigned char)hmax; f.vmax = (unsigned char)vmax;
-      f.mcux = (unsigned)((W + 8 * hmax - 1) / (8 * hmax)); f.mcuy = (unsigned)((H + 8 * vmax - 1) / (8 * vmax));
-      unsigned off = 0;
-      for (int i = 0; i < nc; ++i) {
-        f.w2[i] = f.mcux * f.ch[i] * 8; f.h2[i] = f.mcuy * f.cv[i] * 8;
-        f.cy[i] = (unsigned)((H * f.cv[i] + vmax - 1) / vmax);
-        f.plane_off[i] = off; off += (f.w2[i] * f.h2[i] + 15u) & ~15u;
-      }
-      have_frame = true;
-    } else if (m == 0xC2 || (m >= 0xC3 && m <= 0xCF && m != 0xC4 && m != 0xC8 && m != 0xCC)) { return; }   // progressive / lossless / arithmetic
-    else if (m == 0xDA) {
-      if (!have_frame || sl < 1) return;
-      const int ns = s[0];
-      if (ns != f.ncomp || sl < (size_t)(1 + 2 * ns + 3)) return;
-      for (int i = 0; i < ns; ++i) {
-        if (s[1 + 2 * i] != ids[i]) return;                       // component order of the frame header (what every encoder writes)
-        f.td[i] = s[2 + 2 * i] >> 4; f.ta[i] = s[2 + 2 * i] & 15;
-        if (f.td[i] > 1 || f.ta[i] > 1 || !ts.have_q[f.tq[i]] || !ts.dc[f.td[i]].present || !ts.ac[f.ta[i]].present) return;
-      }
-      if (s[1 + 2 * ns] != 0 || s[3 + 2 * ns] != 0) return;       // spectral start / successive approximation of a sequential scan
-      f.scan_start = (unsigned)(pos + len);
-      f.n_bytes = (unsigned)n;
-      f.supported = 1;
-      out.ok = true;
-      return;
-    }
-    pos += len;
+  Header h(want_w, want_h); Scan sc;
+  if (parse_header(d, n, 2, h, sc, &out.table_bytes) != kScan) return;
+  // the device subset: one baseline / extended-sequential frame header (the parser has already refused Ss, Ah, Al != 0 in it)
+  // and Huffman table ids 0-1
+  if (h.n_sof != 1 || h.sof == 0xC2 || h.other_sof) return;
+  for (int k = 2; k < 4; ++k) if (h.dc[k].present || h.ac[k].present) return;
+  // sampling factors 1 or 2 and 1x1 chroma, so luma carries the full resolution.  A one-component frame is one non-interleaved
+  // scan whatever its sampling factors say: one block per MCU, ceil(W / 8) blocks per row (T.81 A.2.2; jpeg.cpp and stb read it so)
+  const int nc = h.ncomp;
+  for (int i = 0; i < nc; ++i) {
+    const FrameComp& c = h.comp[i];
+    if (c.h > 2 || c.v > 2 || (i > 0 && (c.h != 1 || c.v != 1))) return;
+    f.ch[i] = (unsigned char)(nc == 1 ? 1 : c.h); f.cv[i] = (unsigned char)(nc == 1 ? 1 : c.v); f.tq[i] = (unsigned char)c.tq;
   }
+  // one interleaved scan listing the components in the frame header's order (what every encoder writes; compared by id, as the
+  // stream names them), tables 0-1 present
+  if (sc.ns != nc) return;
+  for (int i = 0; i < nc; ++i) {
+    const int td = sc.td[i], ta = sc.ta[i];
+    if (h.comp[sc.comp[i]].id != h.comp[i].id || td > 1 || ta > 1 || !h.have_q[h.comp[i].tq] || !h.dc[td].present || !h.ac[ta].present) return;
+    f.td[i] = (unsigned char)td; f.ta[i] = (unsigned char)ta;
+  }
+  const int W = h.W, H = h.H, hmax = f.ch[0], vmax = f.cv[0];
+  f.W = (unsigned short)W; f.H = (unsigned short)H; f.ncomp = (unsigned char)nc; f.hmax = (unsigned char)hmax; f.vmax = (unsigned char)vmax;
+  f.restart = (unsigned)h.restart; f.scan_start = (unsigned)sc.data; f.n_bytes = (unsigned)n;
+  f.mcux = (unsigned)((W + 8 * hmax - 1) / (8 * hmax)); f.mcuy = (unsigned)((H + 8 * vmax - 1) / (8 * vmax));
+  unsigned off = 0;
+  for (int i = 0; i < nc; ++i) {
+    f.w2[i] = f.mcux * f.ch[i] * 8; f.h2[i] = f.mcuy * f.cv[i] * 8;
+    f.cy[i] = (unsigned)((H * f.cv[i] + vmax - 1) / vmax);
+    f.plane_off[i] = off; off += (f.w2[i] * f.h2[i] + 15u) & ~15u;
+  }
+  for (int k = 0; k < 2; ++k) { if (h.dc[k].present) ts.dc[k] = h.dc[k]; if (h.ac[k].present) ts.ac[k] = h.ac[k]; }
+  memcpy(ts.quant, h.quant, sizeof(ts.quant));
+  for (int k = 0; k < 4; ++k) ts.have_q[k] = h.have_q[k];
+  f.supported = 1; out.ok = true;
 }
 
 // After the device has consumed the scan: the host decoder would go on reading markers; anything but padding / EOI after
@@ -635,10 +557,7 @@ int scn_jpeg_decode_batch_device(const uint8_t* const* src, const uint64_t* src_
       const int rc = scn::jpeg_decode_rgb8(src[i], (size_t)src_bytes[i], width, height, full.data());
       if (rc) return rc;
       const uint8_t* h = full.data();
-      if (d_lut) {
-        for (uint32_t p = 0; p < out_px; ++p) { const int32_t q = lut[p]; if (q >= 0) { res[3 * (size_t)p] = full[3 * (size_t)q]; res[3 * (size_t)p + 1] = full[3 * (size_t)q + 1]; res[3 * (size_t)p + 2] = full[3 * (size_t)q + 2]; } else res[3 * (size_t)p] = res[3 * (size_t)p + 1] = res[3 * (size_t)p + 2] = 0; }
-        h = res.data();
-      }
+      if (d_lut) { scn::rgb8_through_lut(full.data(), lut.data(), out_px, res.data()); h = res.data(); }
       SCN_CUDA_TRY(cudaMemcpyAsync((uint8_t*)d_out + (size_t)i * out_px * 3, h, (size_t)out_px * 3, cudaMemcpyHostToDevice, st));
       SCN_CUDA_TRY(cudaStreamSynchronize(st));
     }

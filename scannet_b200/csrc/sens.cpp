@@ -27,10 +27,10 @@
 #include <thread>
 #include <vector>
 
+#include "jpeg_common.h"
 #include "scn_common.h"
 
 namespace scn {
-int jpeg_decode_rgb8(const uint8_t* data, size_t n, uint32_t want_w, uint32_t want_h, uint8_t* out);   // jpeg.cpp
 int png_decode_rgb8(const uint8_t* data, size_t n, uint32_t want_w, uint32_t want_h, uint8_t* out);    // jpeg.cpp
 int zlib_inflate(const uint8_t* src, size_t n, std::vector<uint8_t>& out, size_t size_hint);
 void zlib_deflate(const uint8_t* src, size_t n, std::vector<uint8_t>& out);
@@ -798,9 +798,6 @@ int scn::posed_frames(const scn_sens* s, uint64_t f0, uint64_t f1, PosedFrames& 
 
 int scn::sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, size_t n_px, uint8_t* scratch, uint8_t* out) {
   if (int rc = scn_sens_frame_color_rgb8(s, frame, scratch)) return rc;
-  for (size_t p = 0; p < n_px; ++p) {
-    const int32_t q = lut[p]; uint8_t* o = out + 3 * p;
-    if (q >= 0) { o[0] = scratch[3 * (size_t)q]; o[1] = scratch[3 * (size_t)q + 1]; o[2] = scratch[3 * (size_t)q + 2]; } else o[0] = o[1] = o[2] = 0;
-  }
+  rgb8_through_lut(scratch, lut, n_px, out);
   return SCN_OK;
 }
