@@ -249,6 +249,12 @@ int  scn_tsdf_kernel_times(scn_tsdf* t, double* alloc_ms, double* integrate_ms, 
 /* Copies up to `cap` blocks to the host: block_xyz 3*n int32 block coordinates, voxels n*512
  * records of {float sdf; uint8 r,g,b,weight}, x fastest.  Order is heap order (unspecified). */
 int  scn_tsdf_download_blocks(scn_tsdf* t, int32_t* block_xyz, void* voxels, uint64_t cap, uint64_t* n);
+/* The inverse of scn_tsdf_download_blocks: adds n blocks (same layout, HOST buffers) to the volume, block i at heap
+ * index blocks_allocated + i, through the volume's hash so that integration, meshing and reset see them.  Download
+ * followed by upload into a fresh volume of the same parameters restores the volume.  Refused with the volume unchanged:
+ * a coordinate outside [-2^20, 2^20) or a block given twice or already present (SCN_ERR_ARG), more blocks than
+ * max_blocks (SCN_ERR_CAPACITY). */
+int  scn_tsdf_upload_blocks(scn_tsdf* t, const int32_t* block_xyz, const void* voxels, uint64_t n);
 /* Marching-cubes surface of the current volume (malloc'ed; scn_free).  rgb may be NULL. */
 int  scn_tsdf_extract_mesh(scn_tsdf* t, float** xyz, uint8_t** rgb, uint32_t** tri,
                            uint64_t* n_verts, uint64_t* n_faces);

@@ -349,6 +349,38 @@ void oracle_tsdf_export(const oracle_tsdf* o, int32_t* block_xyz, void* voxels) 
   free(ki);
 }
 
+/* The inverse of export: adds n blocks (layout as export) to the volume.  Returns -1 with the volume unchanged when a
+ * coordinate is outside the key range or a block is given twice or already present, else 0. */
+static int64_t find_block(const oracle_tsdf* o, uint64_t key) {
+  uint64_t s = mix64(key) & (o->cap - 1);
+  while (o->keys[s] != EMPTY_KEY && o->keys[s] != key) s = (s + 1) & (o->cap - 1);
+  return o->keys[s] == key ? o->vals[s] : -1;
+}
+int oracle_tsdf_import(oracle_tsdf* o, const int32_t* block_xyz, const void* voxels, uint64_t n) {
+  uint64_t* key = (uint64_t*)malloc((n ? n : 1) * 8);
+  int bad = 0;
+  for (uint64_t i = 0; i < n && !bad; ++i) {
+    const int32_t* b = block_xyz + 3 * i;
+    bad = !key_ok(b[0], b[1], b[2]);
+    if (!bad) { key[i] = pack_key(b[0], b[1], b[2]); bad = find_block(o, key[i]) >= 0; }
+  }
+  if (!bad) {
+    uint64_t* s = (uint64_t*)malloc((n ? n : 1) * 16);
+    for (uint64_t i = 0; i < n; ++i) { s[2 * i] = key[i]; s[2 * i + 1] = i; }
+    qsort(s, n, 16, cmp_u64idx);
+    for (uint64_t i = 1; i < n && !bad; ++i) bad = s[2 * i] == s[2 * i - 2];
+    free(s);
+  }
+  for (uint64_t i = 0; i < n && !bad; ++i) {
+    const int32_t* b = block_xyz + 3 * i;
+    touch_block(o, b[0], b[1], b[2]);                                  /* creates the block (zeroed) */
+    memcpy(o->vox + (size_t)find_block(o, key[i]) * 512, (const char*)voxels + i * 4096, 4096);
+  }
+  o->n_touched = 0;                                                    /* the import is not a frame */
+  free(key);
+  return bad ? -1 : 0;
+}
+
 /* ------------------------------------------------------------------ marching cubes (DESIGN.md §6) -----
  * Own spec (the reference's meshing lives in the external binaries).  Independent statement of the rules
  * the product implements in csrc/mc.cu: usable voxels, valid cubes, lattice-edge vertices, a 256-case

@@ -57,10 +57,10 @@ struct Tables {
 enum { C_HEAP = 0, C_LIST0 = 1, C_LIST1 = 2, C_NU = 3, C_NB = 4, C_ERR = 5, C_UNION = 6, C_WORK0 = 7, C_WORK1 = 8, C_DONE0 = 9, C_DONE1 = 10, C_COUNT = 16 };
 
 // ------------------------------------------------------------------------------ device
-__device__ __forceinline__ bool key_ok(int x, int y, int z) {
+__host__ __device__ __forceinline__ bool key_ok(int x, int y, int z) {
   return x >= -kKeyBias && x < kKeyBias && y >= -kKeyBias && y < kKeyBias && z >= -kKeyBias && z < kKeyBias;
 }
-__device__ __forceinline__ unsigned long long pack_key(int x, int y, int z) {
+__host__ __device__ __forceinline__ unsigned long long pack_key(int x, int y, int z) {
   return (unsigned long long)(unsigned)(x + kKeyBias) | ((unsigned long long)(unsigned)(y + kKeyBias) << 21) |
          ((unsigned long long)(unsigned)(z + kKeyBias) << 42);
 }

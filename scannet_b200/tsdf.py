@@ -129,6 +129,15 @@ class TsdfVolume:
             xyz, vox = xyz[o], vox[o]
         return xyz, vox
 
+    def upload_blocks(self, block_xyz: np.ndarray, voxels: np.ndarray):
+        """Adds blocks (int32 [n,3], VOXEL_DTYPE [n,512], as download_blocks returns them) to the volume."""
+        xyz = np.ascontiguousarray(block_xyz, np.int32).reshape(-1, 3)
+        vox = np.ascontiguousarray(voxels, VOXEL_DTYPE).reshape(-1, 512)
+        if len(xyz) != len(vox):
+            raise ValueError(f"{len(xyz)} block coordinates for {len(vox)} voxel blocks")
+        check(lib().scn_tsdf_upload_blocks(self._h, xyz.ctypes.data_as(C.c_void_p), vox.ctypes.data_as(C.c_void_p),
+                                           C.c_uint64(len(xyz))))
+
 
 def bilateral_filter(depth: np.ndarray, depth_shift: float = 1000.0, sigma_d: float = 2.0, sigma_r: float = 0.05) -> np.ndarray:
     """Depth bilateral pre-filter (scn_depth_bilateral_filter): uint16 [H,W] -> float32 metres, -inf = invalid."""

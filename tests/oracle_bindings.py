@@ -83,6 +83,7 @@ def tsdf_oracle_lib():
         _tsdf.oracle_tsdf_num_blocks.argtypes = [C.c_void_p]
         _tsdf.oracle_tsdf_counters.argtypes = [C.c_void_p, C.c_void_p]
         _tsdf.oracle_tsdf_export.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        _tsdf.oracle_tsdf_import.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         _tsdf.oracle_tsdf_extract_mesh.argtypes = [C.c_void_p, C.c_float] + [C.c_void_p] * 5
         _tsdf.oracle_free.argtypes = [C.c_void_p]
         _tsdf.oracle_mc_table.argtypes = [C.c_void_p, C.c_void_p]
@@ -129,6 +130,15 @@ class OracleTsdf:
         if n:
             tsdf_oracle_lib().oracle_tsdf_export(self._h, xyz.ctypes.data, vox.ctypes.data)
         return xyz, vox
+
+    def import_blocks(self, block_xyz, voxels):
+        """The inverse of export: adds blocks (int32 [n,3], VOXEL_DTYPE [n,512]); raises ValueError, volume unchanged,
+        for a coordinate outside the key range or a block given twice or already present."""
+        xyz = np.ascontiguousarray(block_xyz, np.int32).reshape(-1, 3)
+        vox = np.ascontiguousarray(voxels, VOXEL_DTYPE).reshape(-1, 512)
+        assert len(xyz) == len(vox)
+        if tsdf_oracle_lib().oracle_tsdf_import(self._h, xyz.ctypes.data, vox.ctypes.data, len(xyz)) != 0:
+            raise ValueError("oracle_tsdf_import refused the blocks")
 
     def extract_mesh(self, thresh_factor: float = 10.0):
         L = tsdf_oracle_lib()
