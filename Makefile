@@ -35,6 +35,7 @@ oracle:
 	$(MAKE) -C oracle -f meshclean.mk all
 	$(MAKE) -C oracle -f meshsimplify.mk all
 	$(MAKE) -C oracle -f freespace.mk all
+	$(MAKE) -C oracle -f render.mk all
 
 $(OBJDIR) $(LIBDIR) $(BINDIR):
 	mkdir -p $@

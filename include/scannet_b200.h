@@ -507,6 +507,68 @@ int  scn_freespace_scene(const char* sens_path, const char* out_grid, const scn_
  * params.txt (scn_tsdf_params_from_file) sets the depth range and max_distance; --voxel V sets voxel_size = band_base = V. */
 int  scn_freespace_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Preview render (DESIGN.md §6i): the `render` stage, `python mts_render.py <id>_vh_clean_2.ply` -> `<id>_vh_clean_2.png`
+ * (Server/scan_processor.py:158-160, Server/mts_render.py).  The script path-traces the mesh with Mitsuba, which is not in the
+ * reference tree; the numerics here are this repository's own "render spec v1" and the image is NOT Mitsuba's (box-filtered
+ * hashed samples, two-sided Lambertian surfaces, no Russian roulette, alpha = coverage).  What the script states is kept: argv,
+ * defaults, camera placement, film size, samples, exposure, integrator names and output names.  Tracing runs on the GPU;
+ * there is no CPU fallback.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define SCN_RENDER_PATH 0             /* constant environment of radiance 1, Lambertian surfaces, max_depth interactions */
+#define SCN_RENDER_AO   1             /* one cosine-weighted ray of length ao_length per primary hit: 1 escaped, 0 blocked */
+typedef struct {
+  uint32_t width, height;             /* film size in pixels (640 x 480), 1 .. 16384 each */
+  uint32_t samples;                   /* samples per pixel, 1 .. 256 (16) */
+  int32_t  integrator;                /* SCN_RENDER_PATH (default) or SCN_RENDER_AO */
+  uint32_t max_depth;                 /* path: surface interactions before a path ends with 0, 1 .. 64 (5) */
+  float    exposure;                  /* radiance is scaled by 2^exposure (1.0) */
+  float    world_up[3];               /* (0, 0, 1); the turntable axis and the camera's offset direction */
+  float    camera_up[3];              /* (0, 1, 0); the image's up vector before lookAt */
+  float    camera_offset[3];          /* (0, 0, 0), added to world_up before normalisation (the script leaves its default as is) */
+  float    bsphere_mult;              /* camera distance in bounding-sphere radii (2.5) */
+} scn_render_params;
+/* One view in binary32, made by scn_render_camera.  The sample at film position (fx, fy) (pixel (x, y) covers [x, x+1) x
+ * [y, y+1), y down) has direction p00 + fx*du + fy*dv: du and dv are one pixel right and down, and the component of p00
+ * along the view axis is 1, so t measures depth along that axis for primary rays. */
+typedef struct {
+  float origin[3];
+  float p00[3];                       /* direction through the top-left corner of the film */
+  float du[3], dv[3];
+  float t_near;                       /* primary rays count hits with t > t_near (0.01, Mitsuba's default near clip) */
+  float t_eps;                        /* secondary rays count hits with t > t_eps (2^-16 r) */
+  float ao_length;                    /* length of the ambient-occlusion rays (r, the bounding-sphere radius) */
+} scn_render_camera_t;
+typedef struct scn_render_report {
+  uint64_t views, pixels, samples;    /* per call: views, views*width*height, pixels*samples */
+  uint64_t primary_rays, secondary_rays, primary_hits;   /* equal to the oracle's */
+  uint64_t node_visits, triangle_tests;                  /* BVH inner nodes entered, ray-triangle tests run */
+  uint64_t bvh_nodes;                 /* inner nodes of the tree (faces - 1) */
+  double   upload_ms, bvh_ms, trace_ms, download_ms, total_ms;   /* CUDA events on the call's stream; total: host clock */
+} scn_render_report_t;
+void   scn_render_default_params(scn_render_params* p);
+size_t scn_render_report_sizeof(void);
+/* The camera of one view, from the axis-aligned box of the n_verts vertices (host only, binary64, rounded once): centre c,
+ * radius r = |max - c|, origin = c + bsphere_mult * r * normalize(camera_offset + world_up), lookAt(origin, c, camera_up) with
+ * a 45 degree horizontal field of view.  turntable == 0: origin and camera_up rotated by theta degrees about world_up through
+ * the world origin (the script's single view); turntable != 0: about the axis through c (its turntable frames).
+ * SCN_ERR_ARG: no vertex, a non-finite coordinate, a zero offset + world_up or view direction, camera_up parallel to the
+ * view direction, invalid film size. */
+int  scn_render_camera(const float* xyz, uint64_t n_verts, const scn_render_params* params, double theta, int turntable,
+                       scn_render_camera_t* cam_out);
+/* Renders n_views views of the mesh into rgba_out (caller-owned, n_views * height * width * 4 bytes, view-major, rows top
+ * down): the BVH is built once on the GPU and every (view, pixel, sample) is traced in one launch.  rgb (n_verts*3, sRGB) may
+ * be NULL: reflectance 0.5.  report may be NULL.  SCN_ERR_ARG: no face, a face index >= n_verts, a non-finite coordinate or
+ * one of magnitude > 2^28, invalid parameters or cameras; SCN_ERR_CUDA: no device. */
+int  scn_render_mesh(const float* xyz, const uint8_t* rgb, uint64_t n_verts, const uint32_t* tri, uint64_t n_faces,
+                     const scn_render_params* params, const scn_render_camera_t* cams, uint32_t n_views, uint8_t* rgba_out,
+                     scn_render_report_t* report);
+/* `render [-o out.png] [--integrator path|ao] [--samples N] [--width W] [--height H] [--theta T] [--exposure E]
+ * [--world_up v] [--camera_up v] [--camera_offset v] [--bsphere_mult M] [--render_turntable] [--frames_per_degree D] mesh.ply`:
+ * mts_render.py's arguments.  Writes splitext(mesh)[0] + ".png" (or -o), or with --render_turntable the floor(360 / D) frames
+ * mesh.ply_000.png ... (D degrees apart; no video).  `mlt` and `vpl` give SCN_ERR_UNSUPPORTED, as does --cameras. */
+int  scn_render_main(int argc, const char** argv);
+
 #ifdef __cplusplus
 }
 #endif
