@@ -36,6 +36,7 @@ oracle:
 	$(MAKE) -C oracle -f meshsimplify.mk all
 	$(MAKE) -C oracle -f freespace.mk all
 	$(MAKE) -C oracle -f render.mk all
+	$(MAKE) -C oracle -f track.mk all
 
 $(OBJDIR) $(LIBDIR) $(BINDIR):
 	mkdir -p $@

@@ -569,6 +569,74 @@ int  scn_render_mesh(const float* xyz, const uint8_t* rgb, uint64_t n_verts, con
  * mesh.ply_000.png ... (D degrees apart; no video).  `mlt` and `vpl` give SCN_ERR_UNSUPPORTED, as does --cameras. */
 int  scn_render_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Camera tracking (DESIGN.md §6j): the tracker of the `recons` stage, `FriedLiver.exe <params.txt> <params2.txt> <id>.sens`
+ * (Server/scan_processor.py:27-29,123-126).  BundleFusion is not in the reference tree; this is the repository's own "tracking spec
+ * v1", a frame-to-model dense point-to-plane ICP of the kind VoxelHashing's DepthSensing runs (no sparse features, no global
+ * optimisation, no relocalisation): NOT BundleFusion's trajectory.  Every frame is tracked against a raycast of the volume, then
+ * integrated into it at its tracked pose.  Tracking runs on the GPU; there is no CPU fallback.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct scn_track scn_track;
+typedef struct {
+  uint32_t width, height;             /* tracking / raycast resolution (s_rayCastWidth/Height 320 x 240): the volume's depth
+                                         resolution divided by a power of two */
+  float    dist_thresh;               /* s_projCorrDistThres (0.15 m): largest |Tp - q| of a pair */
+  float    normal_thresh;             /* s_projCorrNormalThres (0.95): smallest n(Tp) . n_q of a pair */
+  float    ray_increment_factor;      /* s_SDFRayIncrementFactor (0.8): raycast step in units of the volume's trunc_base */
+} scn_track_params;
+typedef struct {
+  float    cam2world[16];             /* tracked pose; all -inf when the frame was lost (sensorData.h:382) */
+  uint32_t iterations[3];             /* Gauss-Newton iterations run per level, finest first */
+  uint32_t pairs;                     /* pairs of the last system solved */
+  uint32_t valid_pixels;              /* frame pixels with a vertex and a normal at the finest level */
+  uint32_t lost;                      /* 1: not integrated, pose invalid */
+  double   residual_ss, rms;          /* sum of r^2 of the last system, sqrt(residual_ss / pairs) */
+} scn_track_frame_t;
+void   scn_track_default_params(scn_track_params* p);
+/* `key = value;` parameter files (zParametersScanNet.txt, zParametersBundlingScanNet.txt): the keys above; others are ignored */
+int    scn_track_params_from_file(const char* path, scn_track_params* p);
+size_t scn_track_frame_sizeof(void);
+/* A tracker bound to `vol` (its depth resolution, range, truncation, filter and stream).  SCN_ERR_ARG: a tracking resolution that
+ * is not the depth resolution divided by a power of two, or below 12 x 12. */
+int    scn_track_create(scn_tsdf* vol, const scn_track_params* p, scn_track** out);
+void   scn_track_destroy(scn_track* t);
+/* Tracks and integrates n frames whose depth (n * W * H u16) and colour (n * W * H RGB8 registered to the depth image, or NULL)
+ * live in DEVICE memory, one after the other: each is tracked against the model of the last integrated frame, then integrated
+ * into the volume at its tracked pose and the model is raycast from there.  The first frame of the tracker takes first_pose when
+ * it is finite, identity otherwise; later calls continue the same trajectory.  out[i] per frame.  Returns SCN_ERR_CAPACITY when
+ * the volume's heap or table ran full. */
+int    scn_track_frames(scn_track* t, uint32_t n, const uint16_t* d_depth, const uint8_t* d_rgb, const float K[16], const float first_pose[16],
+                        scn_track_frame_t* out);
+/* frames tracked and kernels launched so far (tracking, raycast and the volume's integration) */
+int    scn_track_stats(const scn_track* t, uint64_t* frames, uint64_t* kernel_launches);
+/* GPU time so far by phase, milliseconds from CUDA events on the volume's stream: depth to metres + filter + pyramids + frame maps;
+ * the ICP iterations and the pose; the volume's integration; raycast + model maps.  Any pointer may be NULL. */
+int    scn_track_phase_ms(const scn_track* t, double* frame_maps_ms, double* icp_ms, double* integrate_ms, double* raycast_ms);
+
+/* The `recons` stage: every frame of the .sens (depth and JPEG colour decoded on the GPU, colour registered as scn_fuse_scene does)
+ * tracked and integrated into a new volume, then marching cubes -> out_ply (NULL: no mesh) and the tracked poses (-inf for a lost
+ * frame) written into out_sens (NULL: the input, replaced atomically); only the 64-byte pose fields differ from the input.
+ * params' width, height and depth_shift come from the stream.  Nothing is written when the call fails (SCN_ERR_IO: the .sens
+ * cannot be read; SCN_ERR_CAPACITY: the volume's heap or table ran full; SCN_ERR_ARG: see scn_track_create).  report may be NULL. */
+typedef struct scn_recons_report {
+  int32_t  status, device;
+  uint64_t frames, frames_tracked, frames_lost;
+  uint64_t blocks_allocated, mesh_vertices, mesh_faces;
+  uint64_t kernel_launches;
+  double   setup_s;                    /* open the file, create the volume and the tracker */
+  double   recons_s;                   /* first frame decoded -> last frame integrated */
+  double   decode_s, track_s;          /* of recons_s: depth + colour decode; tracking + integration (host clock) */
+  double   filter_pyramid_ms, icp_ms, integrate_ms, raycast_ms;   /* of track_s: CUDA events (scn_track_phase_ms) */
+  double   mc_s, ply_s, sens_s, total_s;   /* marching cubes, PLY write, .sens write, everything */
+} scn_recons_report_t;
+size_t scn_recons_report_sizeof(void);
+int    scn_recons_scene(const char* sens_path, const char* out_ply, const char* out_sens, const scn_tsdf_params* params,
+                        const scn_track_params* tparams, int device, scn_recons_report_t* report);
+/* `recons <params.txt> <params2.txt> <file.sens> [out.ply]` (the RECONS_BIN contract, Server/scan_processor.py:27-29): both files
+ * are read for the volume and the tracker; writes <base>.ply beside the input unless an output is given, and the trajectory into
+ * the .sens. */
+int    scn_recons_main(int argc, const char** argv);
+
 #ifdef __cplusplus
 }
 #endif

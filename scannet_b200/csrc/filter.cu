@@ -93,6 +93,15 @@ int scn_filter_batch(scn_tsdf* t, int n, const uint16_t* d_depth, const BatchPar
   return SCN_OK;
 }
 
+// one frame of device depth -> metres (-inf invalid), bilateral-filtered into d_out when `filter` (d_raw is scratch), on `st`
+int scn_depth_to_metres_device(const uint16_t* d_depth, int W, int H, float depth_shift, bool filter, float sd, float sr, float* d_raw,
+                               float* d_out, cudaStream_t st) {
+  const size_t px = (size_t)W * H;
+  BatchParams bp; bp.n = 1; bp.f[0].src = 0;
+  k_depth_to_metres_minf<<<dim3((unsigned)((px + 255) / 256), 1), 256, 0, st>>>(d_depth, bp, depth_shift, px, filter ? d_raw : d_out);
+  return filter ? launch_filter(d_raw, d_out, W, H, 1, sd, sr, st) : SCN_OK;
+}
+
 extern "C" int scn_depth_bilateral_filter(const uint16_t* depth, uint32_t w, uint32_t h, float depth_shift, float sigma_d, float sigma_r,
                                           float* out_metres) {
   if (!depth || !out_metres || !w || !h || !(depth_shift > 0.f)) return scn::fail(SCN_ERR_ARG, "bad argument");

@@ -66,19 +66,6 @@ struct FirstFailure {
 
 using scn::now_s;
 
-// colour pixel for every depth pixel: K_c * K_d^-1 * (x, y, 1), nearest (sensorData.h:1577-1586 with identity extrinsics)
-void build_color_lut(const scn_sens_info_t& in, std::vector<int32_t>& lut) {
-  const uint32_t W = in.depth_width, H = in.depth_height;
-  lut.resize((size_t)W * H);
-  const float fxd = in.depth_intrinsic[0], cxd = in.depth_intrinsic[2], fyd = in.depth_intrinsic[5], cyd = in.depth_intrinsic[6];
-  const float fxc = in.color_intrinsic[0], cxc = in.color_intrinsic[2], fyc = in.color_intrinsic[5], cyc = in.color_intrinsic[6];
-  for (uint32_t y = 0; y < H; ++y) for (uint32_t x = 0; x < W; ++x) {
-    const float u = ((float)x - cxd) / fxd * fxc + cxc, v = ((float)y - cyd) / fyd * fyc + cyc;
-    const long cx = lrintf(u), cy = lrintf(v);
-    lut[(size_t)y * W + x] = (cx >= 0 && cy >= 0 && cx < (long)in.color_width && cy < (long)in.color_height) ? (int32_t)(cy * in.color_width + cx) : -1;
-  }
-}
-
 void decode_chunk(const scn_sens* s, const scn_sens_info_t& in, const std::vector<int32_t>& lut, bool use_color, uint64_t f0, uint32_t n, Chunk& c, Pool& pool,
                   FirstFailure& fail) {
   const size_t px = (size_t)in.depth_width * in.depth_height;
@@ -163,7 +150,7 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
     vs->vol = vol; vs->p = p;
   }
   const size_t px = (size_t)in.depth_width * in.depth_height;
-  std::vector<int32_t> lut; if (use_color) build_color_lut(in, lut);
+  std::vector<int32_t> lut; if (use_color) scn::build_color_lut(in, lut);
   // decode mode
   const bool gpu_able = in.depth_compression == 0 || in.depth_compression == 1;
   const bool gpu_decode = gpu_able && !(job.decode_mode && !strcmp(job.decode_mode, "host"));

@@ -37,6 +37,9 @@ struct PosedFrames { std::vector<uint64_t> frames; std::vector<float> poses; }; 
 int posed_frames(const scn_sens* s, uint64_t f0, uint64_t f1, PosedFrames& out);
 // Decodes the colour of `frame` into `scratch` (color_width x color_height RGB8) and registers it to the depth image:
 // out[p] = scratch[lut[p]], black where lut[p] < 0, for the n_px depth pixels.
+// Colour pixel for every depth pixel (row-major, -1 = outside the colour image): K_c * K_d^-1 * (x, y, 1), nearest
+// (sensorData.h:1577-1586 with identity extrinsics).
+void build_color_lut(const scn_sens_info_t& in, std::vector<int32_t>& lut);
 int sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, size_t n_px, uint8_t* scratch, uint8_t* out);
 // The depth of frames[0..n) into device memory, frame after frame (u16, row-major): zlib streams through the GPU inflate, raw
 // frames uploaded.  Returns when the frames are on the device.

@@ -796,6 +796,18 @@ int scn::posed_frames(const scn_sens* s, uint64_t f0, uint64_t f1, PosedFrames& 
   return SCN_OK;
 }
 
+void scn::build_color_lut(const scn_sens_info_t& in, std::vector<int32_t>& lut) {
+  const uint32_t W = in.depth_width, H = in.depth_height;
+  lut.resize((size_t)W * H);
+  const float fxd = in.depth_intrinsic[0], cxd = in.depth_intrinsic[2], fyd = in.depth_intrinsic[5], cyd = in.depth_intrinsic[6];
+  const float fxc = in.color_intrinsic[0], cxc = in.color_intrinsic[2], fyc = in.color_intrinsic[5], cyc = in.color_intrinsic[6];
+  for (uint32_t y = 0; y < H; ++y) for (uint32_t x = 0; x < W; ++x) {
+    const float u = ((float)x - cxd) / fxd * fxc + cxc, v = ((float)y - cyd) / fyd * fyc + cyc;
+    const long cx = lrintf(u), cy = lrintf(v);
+    lut[(size_t)y * W + x] = (cx >= 0 && cy >= 0 && cx < (long)in.color_width && cy < (long)in.color_height) ? (int32_t)(cy * in.color_width + cx) : -1;
+  }
+}
+
 int scn::sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, size_t n_px, uint8_t* scratch, uint8_t* out) {
   if (int rc = scn_sens_frame_color_rgb8(s, frame, scratch)) return rc;
   rgb8_through_lut(scratch, lut, n_px, out);

@@ -175,3 +175,6 @@ inline int read_counters(const scn_tsdf* t, Counters& out) {
 
 // filter.cu: u16 -> metres (-inf invalid) -> bilateral filter for the n frames of a batch, on the allocation stream
 int scn_filter_batch(scn_tsdf* t, int n, const uint16_t* d_depth, const scn_tsdf_detail::BatchParams& bp, int parity, const float** out);
+// filter.cu: one frame u16 -> metres (-inf invalid) [-> bilateral filter] on `st` (the tracker's input, track.cu)
+int scn_depth_to_metres_device(const uint16_t* d_depth, int W, int H, float depth_shift, bool filter, float sd, float sr, float* d_raw,
+                               float* d_out, cudaStream_t st);

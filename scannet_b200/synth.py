@@ -207,6 +207,20 @@ class BoxRoomScene:
         T[:3, 0], T[:3, 1], T[:3, 2], T[:3, 3] = right, down, fwd, pos
         return T.astype(np.float32)
 
+    def orbit_pose(self, i: int, n: int, radius: float = 1.6, height: float = 1.6, target_z: float = 0.7) -> np.ndarray:
+        """Frame i of n on a circle of `radius` around the room's vertical axis, looking at the axis at height target_z: every view
+        holds spheres, floor and walls at several orientations, so all six degrees of freedom of a camera pose are observable
+        from depth alone (camera_pose's outward views often see one wall only)."""
+        t = 2.0 * np.pi * (i / max(n, 1))
+        ctr = self.size / 2.0
+        pos = np.array([ctr[0] + radius * np.cos(t), ctr[1] + radius * np.sin(t), height])
+        fwd = np.array([ctr[0], ctr[1], target_z]) - pos; fwd /= np.linalg.norm(fwd)
+        right = np.cross(fwd, [0.0, 0.0, 1.0]); right /= np.linalg.norm(right)
+        down = np.cross(fwd, right)
+        T = np.eye(4)
+        T[:3, 0], T[:3, 1], T[:3, 2], T[:3, 3] = right, down, fwd, pos
+        return T.astype(np.float32)
+
     def render(self, cam2world: np.ndarray, noise_mm: float = 0.0, drop: float = 0.0, frame_seed: int = 0):
         T = cam2world.astype(np.float64)
         R, o = T[:3, :3], T[:3, 3]
