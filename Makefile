@@ -37,6 +37,7 @@ oracle:
 	$(MAKE) -C oracle -f freespace.mk all
 	$(MAKE) -C oracle -f render.mk all
 	$(MAKE) -C oracle -f track.mk all
+	$(MAKE) -C oracle -f globalopt.mk all
 
 $(OBJDIR) $(LIBDIR) $(BINDIR):
 	mkdir -p $@

@@ -637,6 +637,73 @@ int    scn_recons_scene(const char* sens_path, const char* out_ply, const char* 
  * the .sens. */
 int    scn_recons_main(int argc, const char** argv);
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * Global optimisation of the keyframe trajectory (DESIGN.md §6k, "global optimisation spec v1"): the dense geometric term of
+ * BundleFusion's global stage without its sparse features.  Keyframes (one per submap of consecutive frames) are linked by an edge
+ * when they are consecutive or when j's depth overlaps i's at the initial poses; every edge contributes point-to-plane residuals
+ * between the two keyframes' maps, and Gauss-Newton with block-Jacobi PCG moves every keyframe but the first of each connected
+ * component.  Edges whose residual stays high are removed and the solve repeated; a result that still fails is rejected and the
+ * poses handed in stand.  Loop closure is the overlap check alone: a revisit is found only when the drifted poses still fall inside
+ * the association basin (dist_thresh, normal_thresh).  Everything runs on the GPU; there is no CPU fallback.  `recons --global`
+ * (scn_recons_scene_global) runs it inside the `recons` stage.
+ * ------------------------------------------------------------------------------------------------------------------ */
+typedef struct scn_globalopt scn_globalopt;
+typedef struct {
+  uint32_t submap_size;               /* s_submapSize (10): frames per submap; its first tracked frame is the keyframe */
+  uint32_t max_keyframes;             /* s_maxNumImages (2000), at most 65535 (one grid row of the overlap check per keyframe) */
+  uint32_t width, height;             /* s_downsampledWidth/Height (80 x 60): the depth resolution divided by a power of two */
+  float    dist_thresh;               /* s_denseDistThresh (0.15 m) */
+  float    normal_thresh;             /* s_denseNormalThresh (0.95) */
+  float    depth_min, depth_max;      /* s_denseDepthMin/Max (0.5, 4.0 m): the range test of the keyframe depth */
+  uint32_t overlap_subsample;         /* s_denseOverlapCheckSubsampleFactor (4) */
+  uint32_t nonlin_iters;              /* s_numGlobalNonLinIterations (3), at most 16 */
+  uint32_t lin_iters;                 /* s_numGlobalLinIterations (150) */
+  float    verify_thresh;             /* s_verifyOptErrThresh (0.05 m): largest edge RMS at the final poses */
+  uint32_t max_removed;               /* s_maxNumResidualsRemoved (10) */
+} scn_globalopt_params;
+typedef struct {
+  uint32_t keyframes, edges_consecutive, edges_loop, edges_removed, rejected;
+  uint32_t solves;                    /* 1 + edges removed */
+  uint32_t nonlin_iterations, lin_iterations;   /* Gauss-Newton and PCG iterations run over all solves */
+  uint64_t pairs_before, pairs_after; /* pairs over the edges at the poses handed in / at the final poses */
+  double   rss_before, rss_after, rms_before, rms_after;
+  double   max_edge_rms;              /* largest edge RMS at the final poses */
+  double   rss_iter[16];              /* sum of r^2 at the start of each Gauss-Newton iteration of the last solve */
+  double   keyframe_maps_ms, overlap_ms, linearise_ms, pcg_ms, verify_ms;   /* GPU time, CUDA events */
+} scn_globalopt_report_t;
+typedef struct {
+  uint32_t i, j, loop, removed;       /* loop: not consecutive keyframes; removed by verification */
+  uint32_t pairs;                     /* at the final poses (0 once removed) */
+  uint32_t pad_;
+  double   rss, rms;
+} scn_globalopt_edge_t;
+void   scn_globalopt_default_params(scn_globalopt_params* p);
+/* `key = value;` parameter files (zParametersBundlingScanNet.txt): the keys above; others are ignored */
+int    scn_globalopt_params_from_file(const char* path, scn_globalopt_params* p);
+size_t scn_globalopt_report_sizeof(void);
+/* An optimiser bound to `vol` (its depth resolution, depth shift, filter and stream).  SCN_ERR_ARG: a keyframe resolution that is not
+ * the depth resolution divided by a power of two, or below 3 x 3, or other parameters out of range. */
+int    scn_globalopt_create(scn_tsdf* vol, const scn_globalopt_params* p, scn_globalopt** out);
+void   scn_globalopt_destroy(scn_globalopt* g);
+/* Adds n keyframes whose depth (n * W * H u16) lives in DEVICE memory and whose cam2world poses (n * 16) are on the host; K is the
+ * depth intrinsic.  SCN_ERR_CAPACITY when the keyframes would exceed max_keyframes (none of the n is added). */
+int    scn_globalopt_add_keyframes(scn_globalopt* g, uint32_t n, const uint16_t* d_depth, const float* poses, const float K[16]);
+/* Solves the keyframes added so far: poses_out (keyframes * 16) receives the optimised cam2world, or the poses handed in when the
+ * result is rejected.  report may be NULL. */
+int    scn_globalopt_solve(scn_globalopt* g, float* poses_out, scn_globalopt_report_t* report);
+/* The edges of the last solve in (i, j) order: writes min(n, cap) entries and the edge count to *n. */
+int    scn_globalopt_edges(const scn_globalopt* g, scn_globalopt_edge_t* out, uint32_t cap, uint32_t* n);
+/* The `recons` stage with the global optimisation (`recons --global`): scn_recons_scene's tracking, and each chunk's keyframes (the
+ * first tracked frame of every submap of gparams->submap_size frames) handed to an optimiser on the tracking volume.  After the
+ * last chunk the keyframes are solved; every other tracked frame follows its submap's keyframe, T_f' = T_k' (T_k^-1 T_f) in binary64
+ * rounded once (lost frames keep -inf); the stream is re-integrated at the new poses into a fresh volume by scn_fuse_scene's driver
+ * (its batch size and decode, params as given), out_ply is written from that volume and then the poses into out_sens.  A rejected
+ * result leaves the output of scn_recons_scene.  Nothing is written when the call fails (SCN_ERR_CAPACITY also for more keyframes
+ * than gparams->max_keyframes).  report and greport may be NULL. */
+int    scn_recons_scene_global(const char* sens_path, const char* out_ply, const char* out_sens, const scn_tsdf_params* params,
+                               const scn_track_params* tparams, const scn_globalopt_params* gparams, int device, scn_recons_report_t* report,
+                               scn_globalopt_report_t* greport);
+
 #ifdef __cplusplus
 }
 #endif

@@ -63,6 +63,10 @@ def lib() -> C.CDLL:
         _lib.scn_host_alloc.argtypes = [C.c_size_t]
         _lib.scn_host_free.argtypes = [C.c_void_p]
         _lib.scn_free.argtypes = [C.c_void_p]
+        _lib.scn_device_alloc.restype = C.c_void_p
+        _lib.scn_device_alloc.argtypes = [C.c_size_t]
+        _lib.scn_device_free.argtypes = [C.c_void_p]
+        _lib.scn_memcpy_h2d.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]
     return _lib
 
 

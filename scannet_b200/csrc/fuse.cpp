@@ -117,6 +117,8 @@ struct FrameBufs {
 scn::StagePool<FrameBufs>& frame_pool() { static auto* p = new scn::StagePool<FrameBufs>(); return *p; }
 scn::StagePool<VolSlot>& vol_pool() { static auto* p = new scn::StagePool<VolSlot>(); return *p; }
 
+int fuse_open_scene(const SceneJob& job, const scn_sens* s, scn_fuse_report_t& rep, double t_begin);
+
 int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
   scn_fuse_report_t rep; memset(&rep, 0, sizeof(rep));
   rep.device = job.device;
@@ -129,7 +131,15 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
   warm.join();
   if (open_rc) return scn::fail(open_rc, "%s", open_err.c_str());
   scn::SensPtr sens(sp);
-  const scn_sens* s = sens.get();
+  const int rc = fuse_open_scene(job, sens.get(), rep, t_begin);
+  sens.reset();                                                // total_s includes unmapping the file
+  rep.total_s = now_s() - t_begin;
+  if (rep_out) *rep_out = rep;
+  return rc;
+}
+
+// The scene of an open stream, with the poses it holds in memory: the volume, the decode and the integration, then the mesh.
+int fuse_open_scene(const SceneJob& job, const scn_sens* s, scn_fuse_report_t& rep, double t_begin) {
   scn_sens_info_t in; scn_sens_info(s, &in);
   scn_tsdf_params p = job.params;
   p.width = in.depth_width; p.height = in.depth_height; p.depth_shift = in.depth_shift;   // integrate at the stream's depth resolution
@@ -311,15 +321,24 @@ int fuse_scene(const SceneJob& job, scn_fuse_report_t* rep_out) {
     }
   }
   if (fail) vs->release();                                     // do not hand a volume of unknown state to the next scene
-  sens.reset();                                                // total_s includes unmapping the file
-  rep.total_s = now_s() - t_begin;
-  if (rep_out) *rep_out = rep;
   return fail ? scn::fail(fail.rc.load(), "%s: %s", job.sens_path.c_str(), fail.err.c_str()) : SCN_OK;
 }
 
 std::string default_out(const std::string& sens_path) { return sens_path.substr(0, sens_path.size() - 5) + "_vh.ply"; }
 
 }  // namespace
+
+int scn::fuse_sens(const scn_sens* s, const char* label, const char* out_ply, const scn_tsdf_params* params, int device, scn_fuse_report_t* report) {
+  SceneJob j; j.sens_path = label; j.out_path = out_ply ? out_ply : ""; j.params = *params; j.device = device; j.verbose = false;
+  scn_fuse_report_t rep; memset(&rep, 0, sizeof(rep));
+  rep.device = device;
+  const double t_begin = now_s();
+  if (int r = scn_set_device(device)) return r;
+  const int rc = fuse_open_scene(j, s, rep, t_begin);
+  rep.total_s = now_s() - t_begin;
+  if (report) *report = rep;
+  return rc;
+}
 
 extern "C" {
 

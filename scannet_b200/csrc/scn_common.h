@@ -44,6 +44,8 @@ int sens_color_to_depth(const scn_sens* s, uint64_t frame, const int32_t* lut, s
 // The depth of frames[0..n) into device memory, frame after frame (u16, row-major): zlib streams through the GPU inflate, raw
 // frames uploaded.  Returns when the frames are on the device.
 int sens_depth_to_device(const scn_sens* s, const uint64_t* frames, uint32_t n, uint16_t* d_out, void* stream);
+// scn_fuse_scene on a stream that is already open, with the poses it holds in memory (fuse.cpp); label names it in errors
+int fuse_sens(const scn_sens* s, const char* label, const char* out_ply, const scn_tsdf_params* params, int device, scn_fuse_report_t* report);
 
 }  // namespace scn
 

@@ -12,6 +12,7 @@
 //   k_raycast + reductions + vertex / normal maps give the model of the next frame.
 #include <cmath>
 
+#include "icp_common.cuh"
 #include "tsdf_internal.cuh"
 
 using namespace scn_tsdf_detail;
@@ -19,20 +20,9 @@ using namespace scn_tsdf_detail;
 namespace {
 
 constexpr int kLevels = 3;
-constexpr int kCta = 256;
-constexpr int kNSum = 28;                          // JtJ upper triangle (21), Jtr (6), sum r^2
 constexpr int kIters[kLevels] = {4, 5, 10};        // finest (0) to coarsest (2)
 constexpr double kExitStep = 1e-5;
-constexpr unsigned kMinPairs = 64;
 constexpr double kMaxRms = 0.02;
-constexpr double kDamp = 0x1p-13;
-
-struct Level {
-  int W, H;
-  float fx, fy, cx, cy, ifx, ify;
-  float* depth; float4* v; float4* n;              // frame
-  float* mdepth; float4* mv; float4* mn;           // model
-};
 
 struct State {                                     // device; one frame's ICP
   double D[12];                                    // current estimate: frame camera -> model camera, 3x4
@@ -44,60 +34,7 @@ struct State {                                     // device; one frame's ICP
   double rss;
 };
 
-struct Thresh { float dist2, normal; };
 struct Pose { float T[16]; };
-
-// ---------------------------------------------------------------------------------------------------------------- pyramid
-__global__ void k_range(const float* __restrict__ m, int n, float dmin, float dmax, float* __restrict__ out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float v = m[i];
-  out[i] = (v >= dmin && v <= dmax) ? v : -INFINITY;
-}
-
-__global__ void k_reduce2(const float* __restrict__ in, int W, int H, float* __restrict__ out) {
-  const int w = W / 2, h = H / 2;
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= w * h) return;
-  const int x = i % w, y = i / w;
-  const float q[4] = {in[(2 * y) * W + 2 * x], in[(2 * y) * W + 2 * x + 1], in[(2 * y + 1) * W + 2 * x], in[(2 * y + 1) * W + 2 * x + 1]};
-  float z[4]; int n = 0;
-#pragma unroll
-  for (int k = 0; k < 4; ++k) { const bool ok = q[k] != -INFINITY; z[k] = ok ? q[k] : 0.0f; n += ok; }
-  out[i] = n ? __fdiv_rn(__fadd_rn(__fadd_rn(z[0], z[1]), __fadd_rn(z[2], z[3])), (float)n) : -INFINITY;
-}
-
-__device__ __forceinline__ float4 backproject(const Level& l, const float* D, int x, int y) {
-  const float d = D[y * l.W + x];
-  if (d == -INFINITY) return make_float4(0.f, 0.f, 0.f, 0.f);
-  return make_float4(__fmul_rn(__fmul_rn(__fsub_rn((float)x, l.cx), l.ifx), d), __fmul_rn(__fmul_rn(__fsub_rn((float)y, l.cy), l.ify), d), d, 1.f);
-}
-
-__global__ void k_vertex_normal(const Level l, const float* __restrict__ D, float4* __restrict__ V, float4* __restrict__ N, unsigned* valid) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= l.W * l.H) return;
-  const int x = i % l.W, y = i / l.W;
-  const float4 c = backproject(l, D, x, y);
-  float4 n = make_float4(0.f, 0.f, 0.f, 0.f);
-  V[i] = c;
-  if (c.w != 0.f && x > 0 && y > 0 && x + 1 < l.W && y + 1 < l.H) {
-    const float4 r = backproject(l, D, x + 1, y), le = backproject(l, D, x - 1, y);
-    const float4 dn = backproject(l, D, x, y + 1), up = backproject(l, D, x, y - 1);
-    if (r.w != 0.f && le.w != 0.f && dn.w != 0.f && up.w != 0.f) {
-      const float ux = __fsub_rn(r.x, le.x), uy = __fsub_rn(r.y, le.y), uz = __fsub_rn(r.z, le.z);
-      const float vx = __fsub_rn(dn.x, up.x), vy = __fsub_rn(dn.y, up.y), vz = __fsub_rn(dn.z, up.z);
-      const float cx = __fsub_rn(__fmul_rn(vy, uz), __fmul_rn(vz, uy));       // dv x du: towards the camera
-      const float cy = __fsub_rn(__fmul_rn(vz, ux), __fmul_rn(vx, uz));
-      const float cz = __fsub_rn(__fmul_rn(vx, uy), __fmul_rn(vy, ux));
-      const float len = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(cx, cx), __fmul_rn(cy, cy)), __fmul_rn(cz, cz)));
-      if (len > 0.f) {
-        n = make_float4(__fdiv_rn(cx, len), __fdiv_rn(cy, len), __fdiv_rn(cz, len), 1.f);
-        if (valid) atomicAdd(valid, 1u);
-      }
-    }
-  }
-  N[i] = n;
-}
 
 // ---------------------------------------------------------------------------------------------------------------- raycast
 __device__ __forceinline__ float lerpf(float p, float q, float a) { return __fadd_rn(__fmul_rn(p, __fsub_rn(1.0f, a)), __fmul_rn(q, a)); }
@@ -150,91 +87,19 @@ __global__ void k_raycast(const Level l, const Tables tb, const Pose P, float dm
 }
 
 // ---------------------------------------------------------------------------------------------------------------- ICP
-__device__ __forceinline__ float dot3(float a0, float a1, float a2, float b0, float b1, float b2) {
-  return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
-}
-
 __device__ bool pair_terms(const Level& l, const Thresh th, const float* Df, int i, double* out) {
 #pragma unroll
   for (int k = 0; k < kNSum; ++k) out[k] = 0.0;
-  const float4 p = l.v[i], np = l.n[i];
-  if (np.w == 0.f) return false;
-  const float tx = __fadd_rn(dot3(Df[0], Df[1], Df[2], p.x, p.y, p.z), Df[3]);
-  const float ty = __fadd_rn(dot3(Df[4], Df[5], Df[6], p.x, p.y, p.z), Df[7]);
-  const float tz = __fadd_rn(dot3(Df[8], Df[9], Df[10], p.x, p.y, p.z), Df[11]);
-  if (!(tz > 0.f)) return false;
-  const float u = rintf(__fadd_rn(__fmul_rn(__fdiv_rn(tx, tz), l.fx), l.cx));
-  const float v = rintf(__fadd_rn(__fmul_rn(__fdiv_rn(ty, tz), l.fy), l.cy));
-  if (!(u >= 0.f && u <= (float)(l.W - 1) && v >= 0.f && v <= (float)(l.H - 1))) return false;
-  const int j = (int)v * l.W + (int)u;
-  const float4 q = l.mv[j], nq = l.mn[j];
-  if (nq.w == 0.f) return false;
-  const float dx = __fsub_rn(tx, q.x), dy = __fsub_rn(ty, q.y), dz = __fsub_rn(tz, q.z);
-  if (!(dot3(dx, dy, dz, dx, dy, dz) <= th.dist2)) return false;
-  const float rnx = dot3(Df[0], Df[1], Df[2], np.x, np.y, np.z);
-  const float rny = dot3(Df[4], Df[5], Df[6], np.x, np.y, np.z);
-  const float rnz = dot3(Df[8], Df[9], Df[10], np.x, np.y, np.z);
-  if (!(dot3(rnx, rny, rnz, nq.x, nq.y, nq.z) >= th.normal)) return false;
-  const float r = dot3(dx, dy, dz, nq.x, nq.y, nq.z);
-  const float J[6] = {__fsub_rn(__fmul_rn(ty, nq.z), __fmul_rn(tz, nq.y)), __fsub_rn(__fmul_rn(tz, nq.x), __fmul_rn(tx, nq.z)),
-                      __fsub_rn(__fmul_rn(tx, nq.y), __fmul_rn(ty, nq.x)), nq.x, nq.y, nq.z};
-  int k = 0;
-#pragma unroll
-  for (int a = 0; a < 6; ++a)
-#pragma unroll
-    for (int b = a; b < 6; ++b) out[k++] = __dmul_rn((double)J[a], (double)J[b]);
-#pragma unroll
-  for (int a = 0; a < 6; ++a) out[k++] = __dmul_rn((double)J[a], (double)r);
-  out[k] = __dmul_rn((double)r, (double)r);
+  Assoc a;
+  if (!associate(l, l.mv, l.mn, th, Df, l.v[i], l.n[i], a)) return false;
+  const float4 nq = a.nq;
+  const float J[6] = {__fsub_rn(__fmul_rn(a.ty, nq.z), __fmul_rn(a.tz, nq.y)), __fsub_rn(__fmul_rn(a.tz, nq.x), __fmul_rn(a.tx, nq.z)),
+                      __fsub_rn(__fmul_rn(a.tx, nq.y), __fmul_rn(a.ty, nq.x)), nq.x, nq.y, nq.z};
+  products28(J, a.r, out);
   return true;
 }
 
-// Cholesky of (JtJ + kDamp * pairs * I) x = -Jtr; false when a pivot is not positive
-__device__ bool solve6(const double* sum, unsigned pairs, double* x) {
-  double A[6][6], L[6][6], y[6];
-  const double lambda = __dmul_rn(kDamp, (double)pairs);
-  int k = 0;
-  for (int a = 0; a < 6; ++a) for (int b = a; b < 6; ++b) { A[a][b] = a == b ? __dadd_rn(sum[k], lambda) : sum[k]; A[b][a] = A[a][b]; ++k; }
-  for (int j = 0; j < 6; ++j) {
-    double s = A[j][j];
-    for (int m = 0; m < j; ++m) s = __dsub_rn(s, __dmul_rn(L[j][m], L[j][m]));
-    if (!(s > 0.0)) return false;
-    L[j][j] = __dsqrt_rn(s);
-    for (int i = j + 1; i < 6; ++i) {
-      double q = A[i][j];
-      for (int m = 0; m < j; ++m) q = __dsub_rn(q, __dmul_rn(L[i][m], L[j][m]));
-      L[i][j] = __ddiv_rn(q, L[j][j]);
-    }
-  }
-  for (int i = 0; i < 6; ++i) {
-    double q = -sum[21 + i];
-    for (int m = 0; m < i; ++m) q = __dsub_rn(q, __dmul_rn(L[i][m], y[m]));
-    y[i] = __ddiv_rn(q, L[i][i]);
-  }
-  for (int i = 5; i >= 0; --i) {
-    double q = y[i];
-    for (int m = i + 1; m < 6; ++m) q = __dsub_rn(q, __dmul_rn(L[m][i], x[m]));
-    x[i] = __ddiv_rn(q, L[i][i]);
-  }
-  return true;
-}
 
-// D <- [Cayley(x[0..2]) | x[3..5]] D, Cayley(w) = ((1 - g.g) I + 2 g g^T + 2 [g]x) / (1 + g.g), g = w / 2
-__device__ void apply_update(double* D, const double* x) {
-  const double g[3] = {__dmul_rn(x[0], 0.5), __dmul_rn(x[1], 0.5), __dmul_rn(x[2], 0.5)};
-  const double gg = __dadd_rn(__dadd_rn(__dmul_rn(g[0], g[0]), __dmul_rn(g[1], g[1])), __dmul_rn(g[2], g[2]));
-  const double den = __dadd_rn(1.0, gg);
-  const double S[9] = {0.0, -g[2], g[1], g[2], 0.0, -g[0], -g[1], g[0], 0.0};
-  double R[9], N[12];
-  for (int i = 0; i < 3; ++i) for (int j = 0; j < 3; ++j)
-    R[3 * i + j] = __ddiv_rn(__dadd_rn(__dadd_rn((i == j) ? __dsub_rn(1.0, gg) : 0.0, __dmul_rn(__dmul_rn(2.0, g[i]), g[j])), __dmul_rn(2.0, S[3 * i + j])), den);
-  for (int i = 0; i < 3; ++i) {
-    for (int j = 0; j < 4; ++j)
-      N[4 * i + j] = __dadd_rn(__dadd_rn(__dmul_rn(R[3 * i], D[j]), __dmul_rn(R[3 * i + 1], D[4 + j])), __dmul_rn(R[3 * i + 2], D[8 + j]));
-    N[4 * i + 3] = __dadd_rn(N[4 * i + 3], x[3 + i]);
-  }
-  for (int i = 0; i < 12; ++i) D[i] = N[i];
-}
 
 // One Gauss-Newton iteration at level k.  Slot c = the 256 pixels [256c, 256c + 256): warps of 32 by a halving tree, the 8 warp sums
 // by a halving tree; the last CTA adds the slots in slot order and solves.
@@ -388,12 +253,7 @@ int frame_maps(scn_track* t, const uint16_t* d_depth, const float K[16]) {
   for (int k = 1; k < kLevels; ++k) k_reduce2<<<grid(t->L[k].W * t->L[k].H), kCta, 0, st>>>(t->L[k - 1].depth, t->L[k - 1].W, t->L[k - 1].H, t->L[k].depth);
   for (int k = 0; k < kLevels; ++k) {
     Level& l = t->L[k];
-    const float sc = 1.0f / (float)(1 << (t->s + k));
-    volatile float fx = K[0] * sc, fy = K[5] * sc, a = K[2] + 0.5f, b = K[6] + 0.5f;
-    volatile float cx = a * sc, cy = b * sc;
-    l.fx = fx; l.fy = fy; l.cx = cx - 0.5f; l.cy = cy - 0.5f;
-    volatile float ifx = 1.0f / l.fx, ify = 1.0f / l.fy;
-    l.ifx = ifx; l.ify = ify;
+    level_intrinsics(l, K, t->s + k);
     k_vertex_normal<<<grid(l.W * l.H), kCta, 0, st>>>(l, l.depth, l.v, l.n, k == 0 ? &t->state.as<State>()->valid : nullptr);
   }
   t->launches += 1 + t->s + (kLevels - 1) + kLevels;
